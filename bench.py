@@ -20,6 +20,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -51,7 +52,10 @@ def parse():
     ap.add_argument('--micro-batch-size', type=int, default=1)
     ap.add_argument('--res', type=int, default=1024)
     ap.add_argument('--text-len', type=int, default=512)
-    ap.add_argument('--layers', type=str, default='19,38', help='double,single block counts (default = Flux-dev)')
+    ap.add_argument('--layers', type=str, default=None,
+                    help='double,single block counts (default: Flux-dev 19,38 from 4 pipeline stages up; 10,20 on 1 or 2 stages, '
+                         'where the full model with AdamW state, 8 bytes per parameter = 95 GB, does not fit 80 GB GPUs). '
+                         'Scaling comparisons across stage counts must pass the same value everywhere')
     ap.add_argument('--no-optimizer', action='store_true', help='diagnostic: skip the optimizer step (INVALID as a bench value)')
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-library-baseline', action='store_true',
@@ -70,7 +74,42 @@ def parse():
                     help='flux stage split: balanced by MEASURED block times (double vs single block, probed before the model is built) or by block count')
     ap.add_argument('--instrumented-steps', type=int, default=2,
                     help='extra steps, after the timed region, with a CUDA event pair around every kernel launch (roofline, shares)')
-    return ap.parse_args()
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last timed step computed (loss, and a fixed seeded sample of the '
+                         'updated parameters of this stage) as DIR/<name>.npy, float32/float64, for output-by-output comparison')
+    a = ap.parse_args()
+    if a.steps < 1:
+        ap.error('--steps must be >= 1')
+    if a.layers is None:
+        a.layers = '19,38' if (a.pp or a.gpus) >= 4 else '10,20'
+    return a
+
+
+DUMP_SAMPLES_PER_TENSOR = 4096        # x ~1000 parameter tensors of the full model: < 16 MB of float32 per stage
+DUMP_MAX_BYTES = 60 << 20             # every file of one --dump-outputs run together
+
+
+def dump_outputs(out_dir, loss, params, stage, stages):
+    """loss of the last timed step (float64) and, for this stage, the same seeded positions of every parameter tensor after
+    that step's optimizer update (float32), concatenated in parameter order.  Called on data-parallel rank 0 only (the
+    replicas of a stage hold the same parameters); the stages share DUMP_MAX_BYTES equally."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    g = torch.Generator().manual_seed(0)
+    parts, left = [], DUMP_MAX_BYTES // 4 // stages
+    for p_ in params:
+        flat = p_.detach().reshape(-1)
+        n = min(flat.numel(), DUMP_SAMPLES_PER_TENSOR, left)
+        if n <= 0:
+            break
+        idx = torch.randint(flat.numel(), (n,), generator=g)
+        parts.append(flat[idx.to(flat.device)].float().cpu())
+        left -= n
+    sample = torch.cat(parts).numpy() if parts else np.zeros(0, np.float32)
+    np.save(os.path.join(out_dir, f'params_sample_stage{stage}.npy'), sample.astype(np.float32))
+    if loss is not None:
+        np.save(os.path.join(out_dir, 'loss.npy'), np.array([loss], dtype=np.float64))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -308,13 +347,37 @@ def synth_micro_batches(a, n, seed, device, pinned):
     return out
 
 
-# calibration of the stage split, measured on 8 B200s in round 2 (profiles/r02_flux_pp8.json): a double block costs 1.32-1.39x
-# a single block; forward : input-gradient pass : weight-gradient pass = 30 : 47 : 23.  A probe outside the plausible band
-# (it runs while the other ranks initialise: one 2-GPU run measured 2.65x and split 17 | 40 blocks, kernel-busy 0.46 | 0.93;
-# the busy fractions of that and of two other runs put the steady-state ratio at 1.2-1.3) falls back to these.
+# fallback calibration of the stage split, used when the probe below fails on every rank or gives an implausible ratio (it
+# runs while the other ranks initialise, so a disturbed probe can read far too high): a double block costs 1.30x a single
+# block; forward : input-gradient pass : weight-gradient pass = 30 : 47 : 23.  These values were taken on earlier hardware
+# and are not measured on H100; the probe replaces them whenever it succeeds.
 CALIBRATED_DOUBLE_OVER_SINGLE = 1.30
 PLAUSIBLE_DOUBLE_OVER_SINGLE = (1.15, 1.45)
 CALIBRATED_FBW = (30, 47, 23)
+
+
+# bf16 activations a block keeps per sample until its weight-gradient pass (no recompute), GB: Flux-dev 1024^2 and
+# Qwen-Image 1024^2 (4352-4608 tokens x 3072) ~0.54, Wan2.1-14B 33 frames 512^2 ~1.8 (from the saved tensors listed in
+# DESIGN.md section 3).  HBM_BUDGET_GB leaves 12 GB of an 80 GB H100 for mailboxes, workspaces and the allocator.
+ACT_GB_PER_BLOCK = {'flux': 0.54, 'qwen': 0.54, 'wan': 1.8}
+HBM_BUDGET_GB = 68.0
+# parameters per block: Flux double 36 D^2 (per stream qkv 3, proj 1, MLP 8, modulation 6) and single 15 D^2 at D = 3072;
+# Wan2.1-14B 14 B / 40 blocks; Qwen-Image 20.4 B / 60 blocks
+PARAMS_PER_BLOCK = {'flux': (36 * 3072 ** 2, 15 * 3072 ** 2), 'wan': (0.35e9, 0.35e9), 'qwen': (0.34e9, 0.34e9)}
+
+
+def inflight_bound(family, n_double, n_single, stages):
+    """micro-batches a stage may hold in the split-backward order so that weights + gradients + AdamW state (8 B per
+    parameter) + held activations stay within HBM_BUDGET_GB; at least 1, at most the planner's default 2 x stages.
+    Taken from the block counts alone (an even share of the parameters, and one block more than an even share for the
+    time-balanced Flux split), so the same bound is known before the split is chosen and used both to choose and to run it.
+    Wan / Qwen-Image pass all their blocks as n_double."""
+    pd, ps = PARAMS_PER_BLOCK[family]
+    params_per_stage = (n_double * pd + n_single * ps) / stages
+    blocks = -(-(n_double + n_single) // stages) + (1 if family == 'flux' else 0)
+    free = HBM_BUDGET_GB - 8.0 * params_per_stage / 1e9
+    per_mb = ACT_GB_PER_BLOCK[family] * max(1, blocks)
+    return max(1, min(2 * stages, int(free // per_mb)))
 
 
 def probe_block_times(device, res, text_len, iters=5):
@@ -503,12 +566,20 @@ def main():
     dp = world // stages
     M, mbs = a.micro_batches, a.micro_batch_size
     fam = FAMILIES[a.family]
-    # auto: the split-backward order from 2 stages up.  The planner's replay of the measured-time split (the same C++ code that
-    # predicted the 8-stage gain over 1F1B to within 1.5 %: 1.226x simulated, 1.212x measured) gives 1.97x / 3.72x / 6.83x for
-    # 2 / 4 / 8 stages against the 1F1B bounds 1.88x / 3.37x / 5.57x at 16 micro-batches.
-    # (2 stages x data parallel keeps the reference's 1F1B order, as measured in profiles/r02_qwen_pp2dp4.json: only that
-    # order lets the gradient all-reduce of a layer start under the last backward pass)
+    # auto: the split-backward order from 2 stages up; the planner's replay gives 1.97x / 3.72x / 6.83x for 2 / 4 / 8 stages
+    # against the 1F1B bounds 1.88x / 3.37x / 5.57x at 16 micro-batches (simulated, not measured on H100).
+    # (2 stages x data parallel keeps the reference's 1F1B order: only that order lets the gradient all-reduce of a layer
+    # start under the last backward pass)
     schedule = ('zb' if stages > 2 or (stages == 2 and dp == 1) else '1f1b') if a.schedule == 'auto' else a.schedule
+    max_inflight = a.max_inflight
+    if not max_inflight and stages > 1 and schedule == 'zb':
+        if a.family == 'flux':
+            nd_, ns_ = (int(x) for x in a.layers.split(','))
+        else:
+            from diffusion_pipe_b200.qwen_image import QWEN_IMAGE_CONFIG
+            from diffusion_pipe_b200.wan import WAN_T2V_14B_CONFIG
+            nd_, ns_ = a.blocks or (WAN_T2V_14B_CONFIG if a.family == 'wan' else QWEN_IMAGE_CONFIG)['num_layers'], 0
+        max_inflight = inflight_bound(a.family, nd_, ns_, stages)
 
     # ---- stage partition: measured block times (Flux: double vs single), block count otherwise ----
     probe = None
@@ -527,7 +598,7 @@ def main():
             tdist.all_reduce(t, op=tdist.ReduceOp.MIN)   # every rank must derive the same split: the least disturbed measurement
             t = t.tolist()
             split, blocks_per_stage, stage_weights, zb_costs, partition_desc = split_from_probe(
-                t, n_double, n_single, stages, M, a.max_inflight)
+                t, n_double, n_single, stages, M, max_inflight)
         else:
             split, blocks_per_stage = flop_balanced_split(n_double, n_single, stages)
             stage_weights = [max(1, b) for b in blocks_per_stage]
@@ -545,7 +616,6 @@ def main():
            'pipeline_schedule': schedule, 'zb_stage_weights': stage_weights}
     if zb_costs is not None:
         cfg['zb_costs'] = zb_costs
-    max_inflight = a.max_inflight or (stages if a.family == 'wan' else 0)     # Wan-14B: 9 GB of activations per micro-batch and stage
     if max_inflight:
         cfg['zb_max_inflight'] = max_inflight
     engine, _, _, _ = initialize(model=pm, config=cfg)
@@ -634,6 +704,8 @@ def main():
     launches0 = ops.LAUNCHES
     ms_dev, loss_dev = timed(dev_batches, False, a.steps)           # `value`: no per-kernel events inside
     launches = ops.LAUNCHES - launches0
+    if a.dump_outputs and engine.grid.get_data_parallel_rank() == 0:
+        dump_outputs(a.dump_outputs, loss_dev if engine.is_last_stage() else None, params, engine.stage_id, stages)
     exposed_reduce = sum(reduce_ms) / max(1, len(reduce_ms)) if reduce_ms else 0.0
     ms_e2e, loss_e2e = timed(host_batches, True, a.steps)
     # the same step again with a CUDA event pair around EVERY kernel launch: per-kernel time, roofline, shares (costs ~3 %)
@@ -676,7 +748,7 @@ def main():
         tdist.all_reduce(red_t, op=tdist.ReduceOp.MAX)
     train_tflop = fam['train_tflop'] * n_blocks / fam['blocks']
 
-    # ---- roofline of the dominant kernel (the tcgen05 GEMM): algorithmic 2MNK per launch / CUDA-event duration ----
+    # ---- roofline of the dominant kernel (the wgmma GEMM): algorithmic 2MNK per launch / CUDA-event duration ----
     roof = None
     busy_local = 0.0
     if prof:
@@ -708,8 +780,7 @@ def main():
         breakdown = [{'MNK_aMN_bMN_epi_acc': list(t), 'n': v[0], 'ms': round(v[1], 2), 'tflops': round(v[2] / v[1] / 1e9, 1)}
                      for t, v in sorted(by_shape.items(), key=lambda kv: -kv[1][1])[:16]]
         try:
-            os.makedirs(os.path.join(ROOT, 'gpurun_out'), exist_ok=True)
-            with open(os.path.join(ROOT, 'gpurun_out', f'bench_gemm_breakdown_{a.family}_rank{rank}.json'), 'w') as f:
+            with open(os.path.join(tempfile.gettempdir(), f'bench_gemm_breakdown_{a.family}_rank{rank}.json'), 'w') as f:
                 json.dump(breakdown, f, indent=1)
         except OSError:
             pass
@@ -719,11 +790,11 @@ def main():
                 peaks = json.load(f)
         except Exception:
             pass
-        peak = peaks.get('bf16_tflops_sustained', 1400.0)
+        peak = peaks.get('bf16_tflops_sustained', 989.0)
         achieved = gemm_fl / gemm_ms / 1e9 if gemm_ms > 0 else 0.0
         traffic = gemm_traffic_from_profile()
-        roof = {'bound': 'tensor', 'kernel': 'gemm_bf16_kernel (tcgen05, all epilogues/layouts)', 'achieved': achieved,
-                'peak': peak, 'peak_source': 'MEASURED_PEAKS.json bf16_tflops_sustained' if peaks else 'fallback 1.4 PF sustained',
+        roof = {'bound': 'tensor', 'kernel': 'gemm_bf16_kernel (wgmma, all epilogues/layouts)', 'achieved': achieved,
+                'peak': peak, 'peak_source': 'MEASURED_PEAKS.json bf16_tflops_sustained' if peaks else 'H100 SXM data sheet, dense bf16 at 700 W',
                 'peak_measured_at_sm_mhz': (peaks.get('clocks_under_load') or {}).get('sm_mhz_median'),
                 'unit': 'TFLOP/s', 'frac': achieved / peak, 'traffic': traffic[0], 'traffic_source': traffic[1],
                 'launches_timed': n_gemm, 'avg_launch_ms': gemm_ms / max(1, n_gemm),
@@ -773,7 +844,7 @@ def main():
                        'parallelism': f'pp{stages}' + (f' x dp{dp}' if dp > 1 else ''), 'partition': partition_desc,
                        'activation_recompute': False, 'train_tflop_per_sample': train_tflop,
                        'optimizer': 'none (diagnostic)' if a.no_optimizer else 'torch.optim.AdamW(fused) bf16, clip 1.0 (fused squared-norm kernel)',
-                       'l2_flush': 'working set (>=24 GB of weights+grads per step) is far larger than the 126 MB L2',
+                       'l2_flush': 'working set (>=24 GB of weights+grads per step) is far larger than the 50 MB L2',
                        'weights': f'random init, layer i seeded {WEIGHT_SEED}+i (identical model for every partition / GPU count)',
                        'stage_link': link_name, 'pipeline_schedule': schedule_name},
             'e2e': {'value': e2e_value, 'unit': 'samples/s', 'h2d_bytes_per_step': h2d, 'd2h_bytes_per_step': 4,

@@ -1,8 +1,8 @@
-"""diffusion-pipe_b200: a Blackwell-native (sm_100a) pipeline-parallel training engine that keeps the
+"""diffusion-pipe_b200: a Hopper-native (sm_90a) pipeline-parallel training engine that keeps the
 plugin/operator surface of tdrussell/diffusion-pipe for its Flux training hot path.
 
 Layout
-  csrc/            hand-written CUDA kernels (tcgen05 / TMA / TMEM) + the C ABI (include/dpipe.h)
+  csrc/            hand-written CUDA kernels (wgmma / TMA / mbarrier) + the C ABI (include/dpipe.h)
   _lib.py          ctypes loader for libdpipe_b200.so (fails loudly when it is missing)
   ops.py           thin tensor-level wrappers over the C ABI
   flux_blocks.py   Flux double/single stream blocks as fused autograd Functions over those ops

@@ -66,7 +66,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise DpipeError(
                 f'{LIB_PATH} is missing: build it with `python tools/build_native.py` '
-                '(or __graft_entry__.build()).  There is no CPU/PyTorch fallback for the sm_100a kernels.')
+                '(or __graft_entry__.build()).  There is no CPU/PyTorch fallback for the sm_90a kernels.')
         l = ctypes.CDLL(LIB_PATH)
         l.dpipe_last_error.restype = ctypes.c_char_p
         l.dpipe_abi_version.restype = c_int

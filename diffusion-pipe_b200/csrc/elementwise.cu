@@ -12,7 +12,7 @@
 // (AdaLayerNormZero, gate*out+residual, RMSNorm(q,k), apply_rotary_emb; reference call sites models/flux.py:502,525)
 // and F.mse_loss in models/base.py:418-436.
 #include "host_util.h"
-#include "sm100_common.cuh"
+#include "sm90_common.cuh"
 
 namespace dpipe {
 

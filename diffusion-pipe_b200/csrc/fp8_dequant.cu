@@ -3,7 +3,7 @@
 // The reference stores the frozen base of a LoRA run as torch.float8_e4m3fn / float8_e5m2 without scales
 // (`transformer_dtype = 'float8'`: models/flux.py:172,203-205, models/qwen_image.py:249-262, utils/common.py:18-20) and
 // lets autocast widen the weight to bf16 inside every nn.Linear.  Every fp8 value is exactly representable in bf16, so the
-// widening is a table lookup; the GEMMs then run on the same tcgen05 kernel as the bf16 path.
+// widening is a table lookup; the GEMMs then run on the same wgmma kernel as the bf16 path.
 //
 // HBM-bound: 1 B read + 2 B written per element.  One thread expands 16 codes (one 16-byte load, two 16-byte stores)
 // through a 256-entry bf16 table in shared memory; the grid is a multiple of the SM count and strides over the matrix.

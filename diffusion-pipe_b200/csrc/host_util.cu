@@ -100,10 +100,10 @@ int num_sms() {
   static int cached[64];
   static bool have[64];
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (!have[dev]) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
     have[dev] = true;
   }
@@ -118,6 +118,7 @@ extern "C" int dpipe_check_device(int dev) {
   cudaDeviceProp prop;
   cudaError_t e = cudaGetDeviceProperties(&prop, dev);
   if (e != cudaSuccess) return dpipe::fail(DPIPE_ECUDA, "cudaGetDeviceProperties(%d): %s", dev, cudaGetErrorString(e));
-  if (prop.major != 10) return dpipe::fail(DPIPE_ENOTSUP, "device %d is sm_%d%d; this library is sm_100a only", dev, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return dpipe::fail(DPIPE_ENOTSUP, "device %d is sm_%d%d; this library is sm_90a only", dev, prop.major, prop.minor);
   return 0;
 }

@@ -8,7 +8,7 @@
 // Replaces nn.Linear(SiLU(temb)) inside diffusers AdaLayerNormZero / AdaLayerNormZeroSingle / AdaLayerNormContinuous
 // (reference call sites models/flux.py:502,525,547) and its autograd backward.
 #include "host_util.h"
-#include "sm100_common.cuh"
+#include "sm90_common.cuh"
 
 namespace dpipe {
 

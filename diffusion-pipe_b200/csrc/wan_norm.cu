@@ -5,13 +5,13 @@
 // WanSelfAttention.forward :137-156 (q = norm_q(q(x)), k = norm_k(k(x)), v = v(x); rope_apply on q and k :41-68 —
 // complex multiply of interleaved pairs in fp32, result cast to bf16 by flash_attention :54-78), WanCrossAttention
 // :171-183 (same without RoPE; k, v from the text context).  Flux / Qwen normalise per head, which fits in the GEMM
-// epilogue (gemm_sm100.cu EPI_QKV_ROPE); a 5120-wide row statistic spans 20 N-tiles and cannot, hence these
+// epilogue (gemm_sm90.cu EPI_QKV_ROPE); a 5120-wide row statistic spans 20 N-tiles and cannot, hence these
 // HBM-bound kernels: one CTA per token row, C/8 threads, 16-byte accesses on both layouts.
 //
 // Algorithmic bytes per token and projection: forward reads 2C (+ 4*128 table bytes per head-row, L2-resident),
 // writes 2C (head-major) + 2C (x_hat, saved for backward); backward reads 2C (dy) + 2C (x_hat), writes 2C.
 #include "host_util.h"
-#include "sm100_common.cuh"
+#include "sm90_common.cuh"
 
 namespace dpipe {
 

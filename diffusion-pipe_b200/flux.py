@@ -1,4 +1,4 @@
-"""Flux model definition on the sm_100a kernels — the drop-in for the reference's models/flux.py.
+"""Flux model definition on the sm_90a kernels — the drop-in for the reference's models/flux.py.
 
 Same plugin surface (models/base.py:348-445 via models/flux.py:153-548): `FluxPipeline(config)` with `name`,
 `checkpointable_layers`, `prepare_inputs(batch, timestep_quantile)`, `to_layers()`, `get_loss_fn()`; the layers speak
@@ -36,7 +36,7 @@ FLUX_DEV_CONFIG = {   # reference: configs/flux_dev_config.json
 # generic pieces
 # =====================================================================================================================
 class LinearFn(torch.autograd.Function):
-    """y = x W^T + b on the tcgen05 GEMM; backward = dgrad + wgrad GEMMs + a column-sum kernel."""
+    """y = x W^T + b on the wgmma GEMM; backward = dgrad + wgrad GEMMs + a column-sum kernel."""
 
     @staticmethod
     def forward(ctx, x, lin):
@@ -329,7 +329,7 @@ class FluxPipeline(PluginSurface):
         if isinstance(dtype, str):
             dtype = {'bfloat16': torch.bfloat16, 'float16': torch.float16, 'float32': torch.float32}[dtype]
         if dtype != torch.bfloat16:
-            raise NotImplementedError('the sm_100a Flux path computes in bf16 (model.dtype must be bfloat16)')
+            raise NotImplementedError('the sm_90a Flux path computes in bf16 (model.dtype must be bfloat16)')
         tcfg = self.model_config.get('transformer_config', None)
         # models/flux.py:174-191: without `transformer_path` the weights are `<diffusers_path>/transformer/*.safetensors`,
         # whose config.json describes the architecture (dev / schnell)
@@ -498,9 +498,9 @@ class FluxPipeline(PluginSurface):
         """LoRA on every Linear of the transformer blocks, everything else frozen (lora.py).  Call before to_layers() /
         the engine is built, as the reference does (train.py:531 precedes :597)."""
         if adapter_config.get('type', 'lora') != 'lora':
-            raise NotImplementedError(f"adapter type {adapter_config.get('type')!r}: only 'lora' is built for the sm_100a path")
+            raise NotImplementedError(f"adapter type {adapter_config.get('type')!r}: only 'lora' is built for the sm_90a path")
         if adapter_config.get('dropout', 0.0):
-            raise NotImplementedError('lora dropout > 0 is not supported on the sm_100a path')
+            raise NotImplementedError('lora dropout > 0 is not supported on the sm_90a path')
         self.adapter_config = dict(adapter_config)
         if self.transformer is not None:
             self._adapt(self.transformer, None)
@@ -521,7 +521,7 @@ class FluxPipeline(PluginSurface):
         if isinstance(dtype, str):
             dtype = {'bfloat16': torch.bfloat16, 'float32': torch.float32}[dtype]
         if dtype != torch.bfloat16:
-            raise NotImplementedError('adapter dtype must be bfloat16 on the sm_100a path')
+            raise NotImplementedError('adapter dtype must be bfloat16 on the sm_90a path')
         lora.attach(module, int(self.adapter_config['rank']), dtype, base_storage_dtype(self.model_config))
         if getattr(self, '_adapter_init', None) is not None:
             FluxPipeline._load_factors(module, self._adapter_init)

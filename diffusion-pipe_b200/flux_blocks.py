@@ -1,7 +1,7 @@
-"""Flux transformer blocks on the sm_100a kernels.
+"""Flux transformer blocks on the sm_90a kernels.
 
 Each block is ONE torch.autograd.Function whose forward and backward are sequences of C-ABI kernel launches
-(ops.py): tcgen05 GEMMs with fused epilogues, the fused attention kernels and the HBM-bound LayerNorm /
+(ops.py): wgmma GEMMs with fused epilogues, the fused attention kernels and the HBM-bound LayerNorm /
 modulation / gate kernels.  Nothing here computes with torch ops except [batch, D]-sized vector glue
 (SiLU of the timestep embedding, dtype casts of reduced gradients) and tensor allocation.
 
@@ -12,7 +12,7 @@ kernels consume as one matrix (q,k,v[,proj_mlp]) are allocated fused and exposed
 The arithmetic (including where bf16 roundings happen under the reference's autocast) is the one restated in
 oracle/flux_ref.py; tests/test_flux_blocks_gpu.py checks both directions against it.
 
-Memory policy (B200, 180 GB): no activation recompute at all — a block saves its bf16 intermediates, including the
+Memory policy (H100, 80 GB): no activation recompute at all — a block saves its bf16 intermediates, including the
 LayerNorm+modulation outputs that feed its GEMMs (~0.54 GB per block per sample at 1024^2; round 1 recomputed those two
 HBM passes per stream in backward: 1.5 % of the step for 2 GB per sample).
 """

@@ -4,7 +4,7 @@ blocks named in adapter_target_modules>)`; train.py:115-133 forces alpha = rank,
 
     y = x W^T + b + (x A^T) B^T          W, b frozen;  A [r, K], B [N, r] trained
 
-**LoRA as a K-extension.**  Both terms are contractions feeding one accumulator, so the adapter rides the SAME tcgen05
+**LoRA as a K-extension.**  Both terms are contractions feeding one accumulator, so the adapter rides the SAME wgmma
 GEMM — and therefore every fused epilogue (QKV->RMSNorm->RoPE scatter, bias+GELU, gate*y+residual, x GELU') — instead
 of a second GEMM plus an elementwise add:
 
@@ -90,7 +90,7 @@ class LoraSite:
 
     def __init__(self, lins, rank, dtype=torch.bfloat16, base_dtype=None):
         if rank % 8:
-            raise ValueError(f'LoRA rank must be a multiple of 8 on the sm_100a path (got {rank})')
+            raise ValueError(f'LoRA rank must be a multiple of 8 on the sm_90a path (got {rank})')
         self.lins, self.r = list(lins), rank
         w0 = self.lins[0].weight
         dev = w0.device

@@ -14,7 +14,7 @@ runtime/pipe/engine.py as recorded in SURVEY.md section 8a rows E3-E11:
   train_batch      returns mean micro-batch loss, averaged over DP and broadcast to every stage      (E10)
 
 Stage links: `DistLink` moves boundary tensors with torch.distributed p2p (gloo on CPU, NCCL on GPUs);
-`IpcLink` (pipe/ipc_link.py) is the B200 path — peer copies into pre-registered slots over NVLink with device-side
+`IpcLink` (pipe/ipc_link.py) is the single-node path — peer copies into pre-registered slots over NVLink with device-side
 flags, no NCCL on the boundary.  Selected by `config['stage_link']` ('auto' picks IpcLink on CUDA).
 """
 import os
@@ -264,7 +264,7 @@ class PipelineEngine:
         if self.pipeline_schedule == 'zb' and self.is_pipe_parallel and self.device.type == 'cuda':
             # the split-backward order lets a stage run ahead of its neighbour, which needs one-sided sends.  NCCL
             # point-to-point operations between two ranks run in issue order on both sides: "send activation k+1" on one
-            # stage and "send gradient k" on the other wait for each other's receive forever (seen on 2 B200s in round 2).
+            # stage and "send gradient k" on the other wait for each other's receive forever (seen on 2 GPUs).
             if self.global_rank == 0:
                 print("pipeline_schedule 'zb' needs the one-sided CUDA-IPC stage link; with torch.distributed p2p on the "
                       "stage boundaries the reference's 1F1B order is used instead", flush=True)

@@ -1,4 +1,4 @@
-"""IpcLink — the B200 stage-boundary transport: CUDA-IPC mailboxes + cudaMemcpyPeerAsync over NVLink + device-side
+"""IpcLink — the single-node stage-boundary transport: CUDA-IPC mailboxes + cudaMemcpyPeerAsync over NVLink + device-side
 sequence flags.  No NCCL on the boundary.  The data path lives in C++ (csrc/stage_exec.cu: dpipe_exec_*): the executor
 walks the stage's instruction stream and runs every Send / Recv itself on its own copy stream and events; this module is
 the HOST control plane only — mailbox allocation, the once-per-step shape / IPC-handle handshake over a gloo side group,

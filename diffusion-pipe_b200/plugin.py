@@ -18,7 +18,7 @@ class PluginSurface:
         dev = torch.device(getattr(self, 'device', 'cpu'))
         return bool(self.model_config.get('device_prepare_inputs', False)) and dev.type == 'cuda' and latents.device.type == 'cpu'
 
-    # ---- block swapping (models/base.py:438-445): not needed on 180 GB parts; the driver calls the prepare_* hooks
+    # ---- block swapping (models/base.py:438-445): not needed on 80 GB parts; the driver calls the prepare_* hooks
     #      around every evaluation (train.py:230-241), so they exist and do nothing, as in BasePipeline ----
     def enable_block_swap(self, blocks_to_swap):
         raise NotImplementedError('Block swapping is not implemented for this model')

@@ -1,4 +1,4 @@
-"""Qwen-Image on the sm_100a kernels — the drop-in for the reference's models/qwen_image.py (SURVEY.md row Q1).
+"""Qwen-Image on the sm_90a kernels — the drop-in for the reference's models/qwen_image.py (SURVEY.md row Q1).
 
 Same plugin surface as the reference's QwenImagePipeline (models/qwen_image.py:177-517): `name`,
 `checkpointable_layers`, `prepare_inputs(batch, timestep_quantile)`, `to_layers()`, `get_loss_fn()`, and layers that
@@ -274,7 +274,7 @@ class QwenImagePipeline(PluginSurface):
         if isinstance(dtype, str):
             dtype = {'bfloat16': torch.bfloat16, 'float16': torch.float16, 'float32': torch.float32}[dtype]
         if dtype != torch.bfloat16:
-            raise NotImplementedError('the sm_100a Qwen-Image path computes in bf16 (model.dtype must be bfloat16)')
+            raise NotImplementedError('the sm_90a Qwen-Image path computes in bf16 (model.dtype must be bfloat16)')
         tcfg = self.model_config.get('transformer_config', None)
         if isinstance(tcfg, str):
             with open(tcfg) as f:

@@ -1,4 +1,4 @@
-"""Wan (t2v) on the sm_100a kernels — the drop-in for the reference's models/wan/wan.py + models/wan/model.py
+"""Wan (t2v) on the sm_90a kernels — the drop-in for the reference's models/wan/wan.py + models/wan/model.py
 (SURVEY.md rows W1-W3).
 
 Same plugin surface as the reference's WanPipeline (models/wan/wan.py:67-411): `name`, `checkpointable_layers`,
@@ -7,7 +7,7 @@ Same plugin surface as the reference's WanPipeline (models/wan/wan.py:67-411): `
 (`blocks.N.self_attn.q.weight`, `blocks.N.modulation`, `head.head.weight`, ...), so checkpoints and `original_name`
 match.
 
-A WanAttentionBlock (models/wan/model.py:242-318) is ONE torch.autograd.Function here: tcgen05 GEMMs with fused bias /
+A WanAttentionBlock (models/wan/model.py:242-318) is ONE torch.autograd.Function here: wgmma GEMMs with fused bias /
 GELU / gated-residual epilogues, the fused attention kernels (self-attention over the video tokens with RoPE,
 cross-attention over the 512 text slots), the LayerNorm+modulation kernels in their "bf16 after every op" mode (the
 block's operands are all bf16 tensors in the reference) and the full-width RMSNorm+RoPE kernels of csrc/wan_norm.cu.
@@ -432,7 +432,7 @@ class WanModel(nn.Module):
         super().__init__()
         cfg = dict(WAN_T2V_14B_CONFIG, **(cfg or {}))
         if cfg['model_type'] not in ('t2v', 'i2v_v2'):
-            raise NotImplementedError(f"Wan model_type {cfg['model_type']!r}: 't2v' and 'i2v_v2' (Wan2.2 I2V) run on the sm_100a path")
+            raise NotImplementedError(f"Wan model_type {cfg['model_type']!r}: 't2v' and 'i2v_v2' (Wan2.2 I2V) run on the sm_90a path")
         if cfg['model_type'] == 'i2v_v2' and cfg['in_dim'] == 16:
             cfg['in_dim'] = 36           # models/wan/configs.py (i2v_A14B): x + mask + y channels
         self.config = cfg
@@ -481,7 +481,7 @@ class InitialLayer(nn.Module):
                 item.requires_grad_(True)
         x, y, t, text_embeddings, text_seq_lens, clip_fea = inputs
         if clip_fea.numel() > 0 or (y.numel() > 0) != (self.model_type == 'i2v_v2'):
-            raise NotImplementedError('Wan2.1 i2v / flf2v conditioning (CLIP image context) is not on the sm_100a path; '
+            raise NotImplementedError('Wan2.1 i2v / flf2v conditioning (CLIP image context) is not on the sm_90a path; '
                                       "model_type 'i2v_v2' expects `y`, 't2v' must not get it")
         if torch.is_floating_point(text_seq_lens) or not torch.is_floating_point(text_embeddings):
             raise NotImplementedError('uncached text encoder (token ids in the pipeline tuple) is not supported: cache_text_embeddings must be true')
@@ -503,7 +503,7 @@ class InitialLayer(nn.Module):
         grid_sizes = torch.tensor([grid] * bs, dtype=torch.long, device=dev)
         seq_lens = torch.full((bs,), L, dtype=torch.long, device=dev)
         if t.dim() != 1:
-            raise NotImplementedError('per-token timesteps (Wan2.2 ti2v) are not on the sm_100a path')
+            raise NotImplementedError('per-token timesteps (Wan2.2 ti2v) are not on the sm_90a path')
         emb = sinusoidal_embedding_1d(self.freq_dim, t.flatten()).unflatten(0, (bs, 1))
         e = linear(emb, self.time_embedding[0])
         e = linear(torch.nn.functional.silu(e), self.time_embedding[2])           # [bs, 1, dim] bf16
@@ -602,7 +602,7 @@ class WanPipeline(PluginSurface):
         if isinstance(dtype, str):
             dtype = {'bfloat16': torch.bfloat16, 'float16': torch.float16, 'float32': torch.float32}[dtype]
         if dtype != torch.bfloat16:
-            raise NotImplementedError('the sm_100a Wan path computes in bf16 (model.dtype must be bfloat16)')
+            raise NotImplementedError('the sm_90a Wan path computes in bf16 (model.dtype must be bfloat16)')
         tcfg = self.model_config.get('transformer_config', None)
         if tcfg is None:
             tcfg = self._find_checkpoint_config()

@@ -1,5 +1,5 @@
 /*
- * dpipe.h — C ABI of libdpipe_b200.so: the sm_100a kernels and the 1F1B stage executor behind the
+ * dpipe.h — C ABI of libdpipe_b200.so: the sm_90a kernels and the 1F1B stage executor behind the
  * reference's Flux training hot path.
  *
  * The reference (tdrussell/diffusion-pipe) has no native code and no FFI of its own: every entry
@@ -26,17 +26,17 @@ extern "C" {
 #define DPIPE_OK 0
 #define DPIPE_EINVAL (-1)   /* bad argument (shape/alignment/enum) */
 #define DPIPE_ECUDA (-2)    /* a CUDA runtime/driver call failed */
-#define DPIPE_ENOTSUP (-3)  /* device is not sm_100 / feature not compiled */
+#define DPIPE_ENOTSUP (-3)  /* device is not sm_90 / feature not compiled */
 #define DPIPE_ESTATE (-4)   /* executor used out of order */
 
 const char* dpipe_last_error(void);
 /* returns the ABI version (bumped on any signature change) */
 int dpipe_abi_version(void);
-/* 0 if device `dev` is an sm_100 part this library can run on */
+/* 0 if device `dev` is an sm_90 part this library can run on */
 int dpipe_check_device(int dev);
 
 /* ------------------------------------------------------------------------------------------ */
-/* Dense bf16 GEMM on tcgen05 tensor cores (TMA -> smem -> tcgen05.mma -> TMEM -> epilogue).    */
+/* Dense bf16 GEMM on wgmma tensor cores (TMA -> smem -> wgmma -> registers -> epilogue).      */
 /*   D[M,N] (fp32 accumulators) = Aop[M,K] * Bop[N,K]^T, then a fused epilogue.                  */
 /* replaces: cuBLASLt via nn.Linear inside the diffusers blocks invoked from                     */
 /*           models/flux.py:502,525 (forward) and their autograd backward (dgrad/wgrad).         */
@@ -81,14 +81,14 @@ typedef struct dpipe_gemm_args {
   const void* gate; int64_t gate_stride; /* bf16 [batch, gate_stride], column n of batch b at gate[b*gate_stride+n] */
   int rows_per_batch;           /* rows of A that belong to one sample (for gate / qkv batch index) */
   int accumulate;               /* STORE only: out = bf16(float(out) + acc) */
-  int cta_group;                /* 1: one CTA per 128x256 tile; 2: CTA pair, 256x256 tile (cta_group::2) */
+  int cta_group;                /* 1 or 2; accepted for ABI compatibility: sm_90a runs one CTA per 128x256 tile either way */
   const dpipe_qkv_epilogue* qkv; /* required for DPIPE_EPI_QKV_ROPE */
 } dpipe_gemm_args;
 
 int dpipe_gemm_bf16(const dpipe_gemm_args* args, void* stream);
 
 /* ------------------------------------------------------------------------------------------ */
-/* Fused attention (FlashAttention-style, head_dim 128, non-causal) on tcgen05 + TMEM.           */
+/* Fused attention (FlashAttention-style, head_dim 128, non-causal) on wgmma + TMA.           */
 /* replaces: torch SDPA dispatched by the diffusers Flux attention processor invoked from        */
 /*           models/flux.py:502,525; flash_attn_varlen_func at models/wan/attention.py:108-122.  */
 /* ------------------------------------------------------------------------------------------ */

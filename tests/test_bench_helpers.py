@@ -13,7 +13,7 @@ sys.path.insert(0, ROOT)
 
 def test_time_balanced_split_prefers_fewer_double_blocks_per_stage():
     import bench
-    # Flux-dev: 19 double + 38 single blocks; a double block costs 1.3x a single block in time (measured 1.32-1.39 on B200)
+    # Flux-dev: 19 double + 38 single blocks; a double block costs 1.3x a single block in time (the calibration value of the stage split)
     for stages in (2, 4, 8):
         split, stage_ms, blocks = bench.time_balanced_split(19, 38, stages, 1.3 * 30.0, 30.0, 16, (30, 40, 30), 0)
         assert len(split) == stages - 1 and sum(blocks) == 57 and all(b > 0 for b in blocks)

@@ -1,4 +1,4 @@
-"""CPU: the FMA-pipe exponential of the attention kernels (`f2_exp2_poly`, csrc/sm100_common.cuh) restated in numpy float32
+"""CPU: the FMA-pipe exponential of the attention kernels (`f2_exp2_poly`, csrc/sm90_common.cuh) restated in numpy float32
 with the coefficients READ FROM THE HEADER, against exp2 in float64: the error bound the header states (1.0e-4 relative,
 far below one bf16 ulp = 3.9e-3, which is all a softmax probability keeps), the exponent assembly for negative and positive
 integer parts, the round-to-nearest split at half-integers, and the clamp.  The kernels themselves are checked on the GPU
@@ -12,7 +12,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _coefficients():
-    src = open(os.path.join(ROOT, 'diffusion-pipe_b200', 'csrc', 'sm100_common.cuh')).read()
+    src = open(os.path.join(ROOT, 'diffusion-pipe_b200', 'csrc', 'sm90_common.cuh')).read()
     body = src[src.index('f32x2 f2_exp2_poly(f32x2 x)'):]
     body = body[:body.index('\n}\n')]
     packs = [float(a) for a, b in re.findall(r'f2_pack\(([-0-9.e]+)f, ([-0-9.e]+)f\)', body)]

@@ -92,7 +92,7 @@ betas = [0.9, 0.99]
 @pytest.mark.parametrize('kind,example', [('flux', 'flux_synthetic.toml'), ('qwen_image', 'qwen_image_synthetic.toml'),
                                           ('wan', 'wan_synthetic.toml')])
 def test_model_registry_and_synthetic_examples_feed_prepare_inputs(kind, example):
-    """every model family with an sm_100a path is reachable from the TOML surface, and its synthetic cached examples have
+    """every model family with an sm_90a path is reachable from the TOML surface, and its synthetic cached examples have
     the keys / shapes its prepare_inputs consumes (CPU: lazy layers, no kernels)"""
     from diffusion_pipe_b200 import data_feed
     cfg = T.set_config_defaults(T.load_toml(os.path.join(ROOT, 'examples', example)))

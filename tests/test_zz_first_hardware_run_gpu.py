@@ -1,5 +1,5 @@
 """GPU tests that were written after the round's GPU budget was spent: their first hardware run is the driver's round-end tier,
-so this file sorts last (`-x` must not let a first-run failure hide the suite that already ran green on B200).  Each has a
+so this file sorts last (`-x` must not let a first-run failure hide the suite that already ran green).  Each has a
 CPU twin on the kernel test doubles that passes.
 
 1. fp8 storage of the frozen base under LoRA (`transformer_dtype = 'float8'`) on the real kernels — the widening kernel

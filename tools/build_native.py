@@ -1,9 +1,9 @@
-"""Builds libdpipe_b200.so (all sm_100a kernels + the C ABI) in-tree with nvcc.
+"""Builds libdpipe_b200.so (all sm_90a kernels + the C ABI) in-tree with nvcc.
 
     python tools/build_native.py [--force] [--verbose]
 
-Objects go to build/ (git-ignored); the shared library lands in diffusion-pipe_b200/ so it travels
-with the gpurun snapshot.  Called by __graft_entry__.build().
+Objects go to build/ (git-ignored); the shared library lands in diffusion-pipe_b200/ next to the
+Python package that loads it.  Called by __graft_entry__.build().
 """
 import argparse
 import concurrent.futures as cf
@@ -16,7 +16,7 @@ CSRC = os.path.join(ROOT, 'diffusion-pipe_b200', 'csrc')
 OUT = os.path.join(ROOT, 'diffusion-pipe_b200', 'libdpipe_b200.so')
 BUILD = os.path.join(ROOT, 'build')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
          '--expt-relaxed-constexpr', '-Xcompiler', '-fPIC', '-I', os.path.join(ROOT, 'include')]
 
 
@@ -53,7 +53,7 @@ def build(force=False, verbose=False):
             if r.returncode != 0:
                 raise RuntimeError('nvcc failed for ' + cmd[-3])
     if jobs or force or not os.path.exists(OUT):
-        cmd = [NVCC, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', OUT] + objs      # (the arch also names the link stub)
+        cmd = [NVCC, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', OUT] + objs      # (the arch also names the link stub)
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)

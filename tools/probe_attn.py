@@ -1,17 +1,17 @@
-"""GPU bring-up probe for the attention kernels (run under gpurun); same structure as probe_gemm.py."""
+"""GPU bring-up probe for the attention kernels: accuracy against fp32 PyTorch and timing, one JSON record per case."""
 import argparse
 import json
 import math
 import os
 import subprocess
 import sys
+import tempfile
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, 'tools'))
 from probe_gemm import _err  # noqa: E402
-
 
 def ref_attn(q, k, v, scale):
     import torch
@@ -114,7 +114,6 @@ def run_case(name):
                     res[f'sdpa_{name}_bwd_ms'] = ts[len(ts) // 2]; res[f'sdpa_{name}_bwd_tflops'] = fl / ts[len(ts) // 2] / 1e9
                 except Exception as ex:  # noqa
                     res[f'sdpa_{name}_err'] = repr(ex)[:200]
-            res['variant'] = os.environ.get('DPIPE_ATTN_BWD', 'default(3)')
             res['rel'] = 0.0; res['bad_frac'] = 0.0
     elif kind == 'perf':
         q = torch.randn(B, H, Lq, 128, device=dev).bfloat16()
@@ -169,7 +168,7 @@ CASES = ['fwd:1x2x256x256', 'fwd:2x3x512x384', 'fwd:1x2x300x200', 'fwd:1x2x1024x
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--case')
-    ap.add_argument('--out', default=os.path.join(ROOT, 'gpurun_out', 'probe_attn.json'))
+    ap.add_argument('--out', default=os.path.join(tempfile.gettempdir(), 'probe_attn.json'), help='JSON file the records are written to')
     a = ap.parse_args()
     if a.case:
         try:
@@ -178,7 +177,7 @@ def main():
             r = {'case': a.case, 'ok': False, 'exception': repr(ex)[:500]}
         print('RESULT ' + json.dumps(r))
         return
-    os.makedirs(os.path.dirname(a.out), exist_ok=True)
+    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
     results = []
     for c in CASES:
         t0 = time.time()

@@ -1,15 +1,16 @@
-"""GPU bring-up probe for the tcgen05 GEMM (run under gpurun):
+"""GPU bring-up probe for the wgmma GEMM:
 
     python tools/probe_gemm.py            # runs every case, each in its own subprocess
     python tools/probe_gemm.py --case NAME
 
-Writes gpurun_out/probe_gemm.json.  Each case compares against torch (fp32 math on the same bf16 inputs).
+Writes probe_gemm.json in the temp directory (--out).  Each case compares against torch (fp32 math on the same bf16 inputs).
 """
 import argparse
 import json
 import os
 import subprocess
 import sys
+import tempfile
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -204,13 +205,12 @@ for cg in (1, 2):
     CASES += [f'perf:{cg}:4608x12288x3072:nt', f'perf:{cg}:4608x3072x12288:nn', f'perf:{cg}:12288x3072x4608:tt',
               f'perf:{cg}:4096x9216x3072:nt', f'perf:{cg}:512x9216x3072:nt']
 
-ALT_MN = ['2048,1024,8192', '1024,8192,1024', '2048,8192,128', '2048,128,1024']
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--case')
-    ap.add_argument('--out', default=os.path.join(ROOT, 'gpurun_out', 'probe_gemm.json'))
+    ap.add_argument('--out', default=os.path.join(tempfile.gettempdir(), 'probe_gemm.json'), help='JSON file the records are written to')
     a = ap.parse_args()
     if a.case:
         try:
@@ -219,7 +219,7 @@ def main():
             r = {'case': a.case, 'ok': False, 'exception': repr(ex)[:500]}
         print('RESULT ' + json.dumps(r))
         return
-    os.makedirs(os.path.dirname(a.out), exist_ok=True)
+    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
     results = []
 
     def spawn(case, env=None):
@@ -239,17 +239,9 @@ def main():
         r = spawn(c)
         results.append(r)
         print(json.dumps(r), flush=True)
-        # descriptor bring-up: if an MN-major case fails, try alternative (kstep, LBO, SBO) encodings
-        if not r.get('ok') and c.split(':')[0] in ('nn', 'tt') and c.endswith('512x768x512') and c.split(':')[1] == '1':
-            for alt in ALT_MN:
-                env = dict(os.environ, DPIPE_DEBUG_MN_DESC=alt)
-                r2 = spawn(c, env)
-                r2['mn_desc'] = alt
-                results.append(r2)
-                print(json.dumps(r2), flush=True)
         with open(a.out, 'w') as f:
             json.dump(results, f, indent=1)
-    nfail = sum(1 for r in results if not r.get('ok') and 'mn_desc' not in r)
+    nfail = sum(1 for r in results if not r.get('ok'))
     print(f'probe_gemm: {len(results)} results, {nfail} failing')
 
 

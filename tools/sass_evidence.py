@@ -1,5 +1,5 @@
-"""Per-kernel SASS evidence for the Blackwell-native claim (B200_PROFILING.md, "What proves a Blackwell-native kernel"):
-counts of the tensor-core (UTC*MMA), tensor-memory (LDTM / STTM), TMA (UTMALDG / UTMASTG / UBLKCP) and legacy (HMMA)
+"""Per-kernel SASS evidence for the sm_90a kernels: counts of the warpgroup tensor-core (HGMMA, from wgmma), TMA
+(UTMALDG / UTMASTG / UBLKCP), mbarrier (SYNCS) and legacy mma.sync (HMMA)
 mnemonics in every kernel of the built library, plus registers / shared memory from the ELF.  No GPU needed.
 
     python tools/sass_evidence.py r01        ->  profiles/r01_sass_evidence.md
@@ -13,9 +13,9 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, 'diffusion-pipe_b200', 'libdpipe_b200.so')
 R = sys.argv[1] if len(sys.argv) > 1 else 'r01'
-PATTERNS = [('UTC*MMA (tcgen05.mma)', r'\bUTC[A-Z]*MMA'), ('LDTM (tcgen05.ld)', r'\bLDTM'), ('STTM (tcgen05.st)', r'\bSTTM'),
+PATTERNS = [('HGMMA (wgmma)', r'\bHGMMA'), ('WARPGROUP (wgmma fence / wait)', r'\bWARPGROUP'),
             ('UTMALDG (TMA load)', r'\bUTMALDG'), ('UTMASTG (TMA store)', r'\bUTMASTG'), ('UBLKCP', r'\bUBLKCP'),
-            ('UTCBAR / SYNCS (mbarrier)', r'\bUTCBAR|\bSYNCS'), ('MUFU.EX2', r'\bMUFU\.EX2'), ('HMMA (legacy)', r'\bHMMA'),
+            ('SYNCS (mbarrier)', r'\bSYNCS'), ('MUFU.EX2', r'\bMUFU\.EX2'), ('HMMA (legacy)', r'\bHMMA\b'),
             ('LDG / STG', r'\bLDG|\bSTG'), ('LDS / STS', r'\bLDS|\bSTS')]
 
 
@@ -55,9 +55,9 @@ def main():
     arch = subprocess.run(['cuobjdump', '-lelf', LIB], capture_output=True, text=True).stdout
     with open(out, 'w') as f:
         f.write(f'# {R}: SASS evidence per kernel (`cuobjdump -sass diffusion-pipe_b200/libdpipe_b200.so`, built with '
-                '`-gencode arch=compute_100a,code=sm_100a`)\n\n')
+                '`-gencode arch=compute_90a,code=sm_90a`)\n\n')
         f.write('ELF images: ' + ', '.join(sorted(set(re.findall(r'sm_\d+a?', arch)))) + '\n\n')
-        f.write('Counts of static instructions.  `UTC*MMA` = `tcgen05.mma`, `LDTM`/`STTM` = `tcgen05.ld`/`st` (TMEM), '
+        f.write('Counts of static instructions.  `HGMMA` = `wgmma.mma_async`, '
                 '`UTMALDG`/`UTMASTG` = TMA tensor copies; `HMMA` would be the legacy `mma.sync` path (none).\n\n')
         cols = [p[0] for p in PATTERNS]
         f.write('| kernel | instr | regs | smem (static) | ' + ' | '.join(cols) + ' |\n')
@@ -65,8 +65,8 @@ def main():
         for k, c in kernels.items():
             reg, sh = usage.get(k, ('', ''))
             f.write(f'| `{demangle(k)}` | {c["instructions"]} | {reg} | {sh} | ' + ' | '.join(str(c[x]) if c[x] else '·' for x in cols) + ' |\n')
-        tc = [demangle(k) for k, c in kernels.items() if c['UTC*MMA (tcgen05.mma)']]
-        f.write(f'\nKernels issuing `tcgen05.mma`: {len(tc)} — ' + ', '.join(f'`{t}`' for t in sorted(set(tc))) + '.\n')
+        tc = [demangle(k) for k, c in kernels.items() if c['HGMMA (wgmma)']]
+        f.write(f'\nKernels issuing `wgmma`: {len(tc)} — ' + ', '.join(f'`{t}`' for t in sorted(set(tc))) + '.\n')
         f.write(f'Kernels with `HMMA`: {sum(1 for c in kernels.values() if c["HMMA (legacy)"])}.\n')
     print('wrote', out, len(kernels), 'kernels')
 

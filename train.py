@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""train.py — the reference's training driver surface (train.py:41-143, 276-974) over the B200-native engine.
+"""train.py — the reference's training driver surface (train.py:41-143, 276-974) over the H100-native engine.
 
     torchrun --nproc-per-node N train.py --config examples/flux_synthetic.toml        (or `deepspeed --num_gpus=N train.py --deepspeed --config ...`)
 
@@ -89,10 +89,10 @@ def set_config_defaults(config):
         if 'alpha' in ac:
             raise NotImplementedError('alpha is forced to rank (as in the reference): remove alpha from the [adapter] table')
         if ac['type'] != 'lora':
-            raise NotImplementedError(f"adapter type '{ac['type']}': only 'lora' is built for the sm_100a path")
+            raise NotImplementedError(f"adapter type '{ac['type']}': only 'lora' is built for the sm_90a path")
         for k in ('exclude_modules', 'fuse_adapters'):
             if ac.get(k):
-                raise NotImplementedError(f"[adapter] {k} is not supported on the sm_100a path: adapters ride the fused GEMM sites of "
+                raise NotImplementedError(f"[adapter] {k} is not supported on the sm_90a path: adapters ride the fused GEMM sites of "
                                           'every Linear of the target blocks (models/base.py:263-303 with the default module set)')
         ac['alpha'] = ac['rank']
         ac['dtype'] = DTYPE_MAP[ac['dtype']] if 'dtype' in ac else mc['dtype']
@@ -153,7 +153,7 @@ class CachedExamples:
         return ex
 
 
-MODEL_TYPES = {   # config['model']['type'] -> (module, class): the model families with an sm_100a path (train.py:431-535)
+MODEL_TYPES = {   # config['model']['type'] -> (module, class): the model families with an sm_90a path (train.py:431-535)
     'flux': ('diffusion_pipe_b200.flux', 'FluxPipeline'),
     'qwen_image': ('diffusion_pipe_b200.qwen_image', 'QwenImagePipeline'),
     'wan': ('diffusion_pipe_b200.wan', 'WanPipeline'),
@@ -164,7 +164,7 @@ def make_model(config):
     import importlib
     model_type = config['model']['type']
     if model_type not in MODEL_TYPES:
-        raise NotImplementedError(f"model type '{model_type}': the sm_100a path covers {sorted(MODEL_TYPES)} "
+        raise NotImplementedError(f"model type '{model_type}': the sm_90a path covers {sorted(MODEL_TYPES)} "
                                   '(SURVEY.md section 8); the other model definitions of the reference are out of scope')
     mod, cls = MODEL_TYPES[model_type]
     return getattr(importlib.import_module(mod), cls)(config)
@@ -393,7 +393,7 @@ def main(argv=None):
 
     if config.get('blocks_to_swap', 0) and is_main:                        # train.py:576-583
         print('blocks_to_swap is ignored: block swapping exists to fit 24 GB parts; this engine keeps the whole stage resident '
-              '(180 GB HBM per GPU)')
+              '(80 GB HBM per GPU)')
     if 'monitoring' in config and is_main:
         print('[monitoring] (wandb) is ignored: metrics go to <run_dir>/metrics.jsonl')
     layers = model.to_layers()
