@@ -122,6 +122,8 @@ SIGNATURES['dpipe_fp8_code_table'] = (c_int, [c_int, c_void_p])
 SIGNATURES['dpipe_grad_sumsq_blocks'] = (c_int, [])
 SIGNATURES['dpipe_grad_sumsq'] = (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int64, c_void_p, c_void_p])
 SIGNATURES['dpipe_grad_scale'] = (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p])
+SIGNATURES['dpipe_adamw_step'] = (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float,
+                                          c_float, c_float, c_float, c_float, c_float, c_void_p])
 SIGNATURES['dpipe_noise_pack'] = (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int64, c_int, c_int,
                                           c_int, c_void_p])
 SIGNATURES['dpipe_exec_create'] = (c_int, [c_int, c_int, ctypes.c_double, ctypes.POINTER(c_void_p)])

@@ -13,6 +13,12 @@
 //                      the input layout or packed 2x2 -> [bs, (h/2)(w/2), 4c] (diffusers `_pack_latents`).
 //                                                                                           replaces models/flux.py:368-378,
 //                                                                                           qwen_image.py:447-455, wan.py:400-404.
+//   adamw_step_multi   one pass of optimi's AdamW over up to 64 (p, g, m, v, c) tensor sets per launch, with Kahan-summed
+//                      bf16 weights when c is given.  Every operation is an IEEE round-to-nearest intrinsic in the order of
+//                      the torch ops it replaces, rounded to the state dtype where a bf16 torch op rounds (no FMA
+//                      contraction): bit-identical to oracle/optim_ref.py adamw_step_emulated.
+//                                                                                           replaces optimi.AdamW.step
+//                                                                                           (train.py:676-678).
 #include <cuda_bf16.h>
 
 #include "host_util.h"
@@ -160,6 +166,148 @@ __global__ void noise_pack_kernel(const float* __restrict__ x1, const float* __r
   }
 }
 
+struct AdamwList {
+  void* p[ST_MAX_TENSORS];
+  const void* g[ST_MAX_TENSORS];
+  void* m[ST_MAX_TENSORS];
+  void* v[ST_MAX_TENSORS];
+  void* c[ST_MAX_TENSORS];     // null: no Kahan compensation for this tensor
+  long long numel[ST_MAX_TENSORS];
+  int dtype[ST_MAX_TENSORS];   // 0 = bf16, 1 = fp32 (all five tensors of a set share it)
+  int n;
+};
+
+struct AdamwScalars {
+  float lr, beta1_comp, beta2_hat, one_minus_beta2_hat, eps, decay;
+};
+
+template <bool BF16>
+__device__ __forceinline__ float to_state(float x) {
+  return BF16 ? __bfloat162float(__float2bfloat16_rn(x)) : x;
+}
+
+// one element; p, m, v, c are exact values of the state dtype on entry and on exit
+template <bool BF16, bool KAHAN>
+__device__ __forceinline__ void adamw_elem(float& p, const float g, float& m, float& v, float& c, const AdamwScalars& s) {
+  p = to_state<BF16>(__fmul_rn(p, s.decay));                                     // p.mul_(1 - lr*wd)
+  const float w = s.beta1_comp;                                                  // m.lerp_(g, w), torch's two-sided form
+  const float d = __fsub_rn(g, m);
+  m = to_state<BF16>(fabsf(w) < 0.5f ? __fadd_rn(m, __fmul_rn(w, d)) : __fsub_rn(g, __fmul_rn(d, __fsub_rn(1.0f, w))));
+  v = to_state<BF16>(__fmul_rn(v, s.beta2_hat));                                 // v.mul_(beta2_hat)
+  v = to_state<BF16>(__fadd_rn(v, __fmul_rn(__fmul_rn(s.one_minus_beta2_hat, g), g)));   // .addcmul_(g, g, 1-beta2_hat)
+  const float den = to_state<BF16>(__fadd_rn(to_state<BF16>(__fsqrt_rn(v)), s.eps));      // v.sqrt().add_(eps)
+  const float upd = __fdiv_rn(__fmul_rn(-s.lr, m), den);                         // addcdiv's value * m / den
+  if (KAHAN) {
+    c = to_state<BF16>(__fadd_rn(c, upd));
+    const float old = p;
+    p = to_state<BF16>(__fadd_rn(p, c));
+    c = to_state<BF16>(__fadd_rn(c, to_state<BF16>(__fsub_rn(old, p))));
+  } else {
+    p = to_state<BF16>(__fadd_rn(p, upd));
+  }
+}
+
+template <bool BF16>
+__device__ __forceinline__ float ld_elem(const void* a, long long j) {
+  return BF16 ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(a)[j]) : reinterpret_cast<const float*>(a)[j];
+}
+
+template <bool BF16>
+__device__ __forceinline__ void st_elem(void* a, long long j, float x) {
+  if (BF16) reinterpret_cast<__nv_bfloat16*>(a)[j] = __float2bfloat16_rn(x);
+  else reinterpret_cast<float*>(a)[j] = x;
+}
+
+template <bool BF16, bool KAHAN>
+__device__ __forceinline__ void adamw_scalar(const AdamwList& tl, int i, long long j, const AdamwScalars& s) {
+  float p = ld_elem<BF16>(tl.p[i], j), m = ld_elem<BF16>(tl.m[i], j), v = ld_elem<BF16>(tl.v[i], j);
+  float c = KAHAN ? ld_elem<BF16>(tl.c[i], j) : 0.f;
+  adamw_elem<BF16, KAHAN>(p, ld_elem<BF16>(tl.g[i], j), m, v, c, s);
+  st_elem<BF16>(tl.p[i], j, p);
+  st_elem<BF16>(tl.m[i], j, m);
+  st_elem<BF16>(tl.v[i], j, v);
+  if (KAHAN) st_elem<BF16>(tl.c[i], j, c);
+}
+
+// one 32-bit word of each of the five 16-byte vectors: two bf16 elements or one fp32 element, updated in place (the
+// vectors stay packed in registers: unpacking all five at once does not fit 64 registers)
+template <bool BF16, bool KAHAN>
+__device__ __forceinline__ void adamw_word(uint32_t& pw, const uint32_t gw, uint32_t& mw, uint32_t& vw, uint32_t& cw,
+                                           const AdamwScalars& s) {
+  if (BF16) {
+    constexpr uint32_t HI = 0xffff0000u;
+    // the results are bf16 values: their fp32 bits end in 16 zeros
+    {   // low halves
+      float p = __uint_as_float(pw << 16), m = __uint_as_float(mw << 16), v = __uint_as_float(vw << 16), c = __uint_as_float(cw << 16);
+      adamw_elem<true, KAHAN>(p, __uint_as_float(gw << 16), m, v, c, s);
+      pw = (pw & HI) | (__float_as_uint(p) >> 16);
+      mw = (mw & HI) | (__float_as_uint(m) >> 16);
+      vw = (vw & HI) | (__float_as_uint(v) >> 16);
+      if (KAHAN) cw = (cw & HI) | (__float_as_uint(c) >> 16);
+    }
+    {   // high halves
+      float p = __uint_as_float(pw & HI), m = __uint_as_float(mw & HI), v = __uint_as_float(vw & HI), c = __uint_as_float(cw & HI);
+      adamw_elem<true, KAHAN>(p, __uint_as_float(gw & HI), m, v, c, s);
+      pw = (pw & ~HI) | __float_as_uint(p);
+      mw = (mw & ~HI) | __float_as_uint(m);
+      vw = (vw & ~HI) | __float_as_uint(v);
+      if (KAHAN) cw = (cw & ~HI) | __float_as_uint(c);
+    }
+  } else {
+    float p = __uint_as_float(pw), m = __uint_as_float(mw), v = __uint_as_float(vw), c = 0.f;
+    adamw_elem<false, false>(p, __uint_as_float(gw), m, v, c, s);
+    pw = __float_as_uint(p); mw = __float_as_uint(m); vw = __float_as_uint(v);
+  }
+}
+
+template <bool BF16, bool KAHAN>
+__device__ __forceinline__ void adamw_tensor(const AdamwList& tl, int i, long long tid, long long nthreads, const AdamwScalars& s) {
+  constexpr int VEC = BF16 ? 8 : 4;            // elements per 16-byte vector
+  constexpr int ESZ = BF16 ? 2 : 4;
+  const long long n = tl.numel[i];
+  const uintptr_t mis = reinterpret_cast<uintptr_t>(tl.p[i]) & 15;
+  const bool same = (reinterpret_cast<uintptr_t>(tl.g[i]) & 15) == mis && (reinterpret_cast<uintptr_t>(tl.m[i]) & 15) == mis &&
+                    (reinterpret_cast<uintptr_t>(tl.v[i]) & 15) == mis &&
+                    (!KAHAN || (reinterpret_cast<uintptr_t>(tl.c[i]) & 15) == mis);
+  if (!same) {                                 // views at different offsets mod 16 B: element-wise loads
+    for (long long j = tid; j < n; j += nthreads) adamw_scalar<BF16, KAHAN>(tl, i, j, s);
+    return;
+  }
+  const int head = (int)(((16 - mis) & 15) / ESZ);   // elements before 16-byte alignment
+  const long long h = head < n ? head : n;
+  if (tid < h) adamw_scalar<BF16, KAHAN>(tl, i, tid, s);
+  const long long nv = (n - h) / VEC;
+  uint4* p4 = reinterpret_cast<uint4*>(static_cast<char*>(tl.p[i]) + h * ESZ);
+  const uint4* g4 = reinterpret_cast<const uint4*>(static_cast<const char*>(tl.g[i]) + h * ESZ);
+  uint4* m4 = reinterpret_cast<uint4*>(static_cast<char*>(tl.m[i]) + h * ESZ);
+  uint4* v4 = reinterpret_cast<uint4*>(static_cast<char*>(tl.v[i]) + h * ESZ);
+  uint4* c4 = KAHAN ? reinterpret_cast<uint4*>(static_cast<char*>(tl.c[i]) + h * ESZ) : nullptr;
+  for (long long j = tid; j < nv; j += nthreads) {
+    uint4 P = p4[j], M = m4[j], V = v4[j], C = KAHAN ? c4[j] : make_uint4(0, 0, 0, 0);
+    const uint4 G = __ldg(g4 + j);
+    adamw_word<BF16, KAHAN>(P.x, G.x, M.x, V.x, C.x, s);
+    adamw_word<BF16, KAHAN>(P.y, G.y, M.y, V.y, C.y, s);
+    adamw_word<BF16, KAHAN>(P.z, G.z, M.z, V.z, C.z, s);
+    adamw_word<BF16, KAHAN>(P.w, G.w, M.w, V.w, C.w, s);
+    p4[j] = P;
+    m4[j] = M;
+    v4[j] = V;
+    if (KAHAN) c4[j] = C;
+  }
+  const long long tail0 = h + nv * VEC;
+  if (tail0 + tid < n) adamw_scalar<BF16, KAHAN>(tl, i, tail0 + tid, s);
+}
+
+__global__ void __launch_bounds__(ST_THREADS, 4) adamw_step_multi_kernel(const AdamwList tl, const AdamwScalars s) {
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long nthreads = (long long)gridDim.x * blockDim.x;
+  for (int i = 0; i < tl.n; ++i) {
+    if (tl.dtype[i] == 1) adamw_tensor<false, false>(tl, i, tid, nthreads, s);
+    else if (tl.c[i]) adamw_tensor<true, true>(tl, i, tid, nthreads, s);
+    else adamw_tensor<true, false>(tl, i, tid, nthreads, s);
+  }
+}
+
 static int fill_list(TensorList& tl, const void* const* ptrs, const int64_t* numels, const int* dtypes, int begin, int n) {
   tl.n = 0;
   for (int i = begin; i < n && tl.n < ST_MAX_TENSORS; ++i) {
@@ -209,6 +357,41 @@ extern "C" int dpipe_grad_scale(const void* const* ptrs, const int64_t* numels, 
       return fail(DPIPE_EINVAL, "dpipe_grad_scale: bad tensor %d..", l * ST_MAX_TENSORS);
     if (tl.n == 0) continue;
     grad_scale_multi_kernel<<<blocks, ST_THREADS, 0, (cudaStream_t)stream>>>(tl, coef);
+    DPIPE_CUDA_CHECK(cudaGetLastError());
+  }
+  return 0;
+}
+
+extern "C" int dpipe_adamw_step(void* const* params, const void* const* grads, void* const* exp_avgs, void* const* exp_avg_sqs,
+                                void* const* kahan_comps, const int64_t* numels, const int* dtypes, int n, float lr,
+                                float beta1_comp, float beta2_hat, float one_minus_beta2_hat, float eps, float decay,
+                                void* stream) {
+  if (n < 0) return fail(DPIPE_EINVAL, "dpipe_adamw_step: n < 0");
+  if (n > 0 && (!params || !grads || !exp_avgs || !exp_avg_sqs || !numels || !dtypes))
+    return fail(DPIPE_EINVAL, "dpipe_adamw_step: null argument");
+  // every tensor is checked before the first launch: a bad argument leaves all tensors untouched
+  for (int i = 0; i < n; ++i) {
+    if (numels[i] < 0) return fail(DPIPE_EINVAL, "dpipe_adamw_step: tensor %d has numel < 0", i);
+    if (dtypes[i] != 0 && dtypes[i] != 1) return fail(DPIPE_EINVAL, "dpipe_adamw_step: tensor %d has dtype %d (0 = bf16, 1 = fp32)", i, dtypes[i]);
+    if (numels[i] == 0) continue;
+    if (!params[i] || !grads[i] || !exp_avgs[i] || !exp_avg_sqs[i]) return fail(DPIPE_EINVAL, "dpipe_adamw_step: tensor %d has a null pointer", i);
+    if (kahan_comps && kahan_comps[i] && dtypes[i] != 0)
+      return fail(DPIPE_EINVAL, "dpipe_adamw_step: tensor %d: Kahan compensation is for bf16 tensors only", i);
+  }
+  const AdamwScalars s{lr, beta1_comp, beta2_hat, one_minus_beta2_hat, eps, decay};
+  int i = 0;
+  while (i < n) {
+    AdamwList tl;
+    tl.n = 0;
+    for (; i < n && tl.n < ST_MAX_TENSORS; ++i) {
+      if (numels[i] == 0) continue;
+      tl.p[tl.n] = params[i]; tl.g[tl.n] = grads[i]; tl.m[tl.n] = exp_avgs[i]; tl.v[tl.n] = exp_avg_sqs[i];
+      tl.c[tl.n] = kahan_comps ? kahan_comps[i] : nullptr;
+      tl.numel[tl.n] = numels[i]; tl.dtype[tl.n] = dtypes[i];
+      ++tl.n;
+    }
+    if (tl.n == 0) continue;
+    adamw_step_multi_kernel<<<dpipe_grad_sumsq_blocks(), ST_THREADS, 0, (cudaStream_t)stream>>>(tl, s);
     DPIPE_CUDA_CHECK(cudaGetLastError());
   }
   return 0;

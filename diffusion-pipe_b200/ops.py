@@ -500,7 +500,7 @@ def mse_loss(out, target, mask=None, want_grad=True):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# optimizer-step tail (gradient norm / clipping) and micro-batch preparation
+# optimizer-step tail (gradient norm / clipping, AdamW step) and micro-batch preparation
 # ---------------------------------------------------------------------------------------------------------------
 _GRAD_DTYPES = {torch.bfloat16: 0, torch.float32: 1}
 
@@ -543,6 +543,41 @@ def grad_scale(tensors, coef):
     check(lib().dpipe_grad_scale(ptrs, numels, dtypes, len(tensors), _ptr(coef), _stream()), 'dpipe_grad_scale')
     _prof_end(_e, 0.0, 'grad_scale')
     LAUNCHES += max(1, (len(tensors) + 63) // 64)
+
+
+def adamw_step(params, grads, exp_avgs, exp_avg_sqs, kahan_comps, *, lr, beta1_comp, beta2_hat, one_minus_beta2_hat, eps,
+               decay):
+    """One AdamW step (optimi's update rule, include/dpipe.h dpipe_adamw_step) in place over the tensor sets
+    (p, g, m, v, c): contiguous CUDA tensors of one shape and dtype (bf16 or fp32) per set; kahan_comps[i] is None for no
+    Kahan compensation and must be None for fp32.  The scalars are the fp32 values the kernel uses (optim.step_scalars)."""
+    global LAUNCHES
+    n = len(params)
+    if not (len(grads) == len(exp_avgs) == len(exp_avg_sqs) == len(kahan_comps) == n):
+        raise ValueError('adamw_step: the five tensor lists differ in length')
+    for i, (p, g, m, v, c) in enumerate(zip(params, grads, exp_avgs, exp_avg_sqs, kahan_comps)):
+        if p.dtype not in _GRAD_DTYPES:
+            raise TypeError(f'adamw_step: tensor {i} is {p.dtype}; the kernel takes bf16 or fp32')
+        for t, name in ((p, 'param'), (g, 'grad'), (m, 'exp_avg'), (v, 'exp_avg_sq'), (c, 'kahan_comp')):
+            if t is None and name == 'kahan_comp':
+                continue
+            if not t.is_cuda or t.dtype != p.dtype or t.shape != p.shape or not t.is_contiguous():
+                raise TypeError(f'adamw_step: {name} {i} must be a contiguous CUDA {p.dtype} tensor of shape '
+                                f'{tuple(p.shape)}, got {t.dtype} {tuple(t.shape)} on {t.device}')
+        if c is not None and p.dtype != torch.bfloat16:
+            raise TypeError(f'adamw_step: tensor {i}: Kahan compensation is for bf16 tensors only')
+    if n == 0:
+        return
+
+    def ptrs(ts):
+        return (ctypes.c_void_p * n)(*[t.data_ptr() if t is not None else None for t in ts])
+    numels = (ctypes.c_int64 * n)(*[p.numel() for p in params])
+    dtypes = (ctypes.c_int * n)(*[_GRAD_DTYPES[p.dtype] for p in params])
+    _e = _prof_begin()
+    check(lib().dpipe_adamw_step(ptrs(params), ptrs(grads), ptrs(exp_avgs), ptrs(exp_avg_sqs), ptrs(kahan_comps), numels,
+                                 dtypes, n, lr, beta1_comp, beta2_hat, one_minus_beta2_hat, eps, decay, _stream()),
+          'dpipe_adamw_step')
+    _prof_end(_e, 0.0, 'adamw_step')
+    LAUNCHES += (n + 63) // 64
 
 
 def noise_pack(x1, x0, t, pack):

@@ -245,6 +245,19 @@ int dpipe_grad_sumsq(const void* const* ptrs, const int64_t* numels, const int* 
  * replaces: `p.grad.data.mul_(clip_coef)` (utils/patches.py:238-243). */
 int dpipe_grad_scale(const void* const* ptrs, const int64_t* numels, const int* dtypes, int n, const float* coef,
                      void* stream);
+/* One AdamW step with optimi's update rule over n tensor sets (p, g, m, v, c) of numels[i] elements each, all five of
+ * dtypes[i] (0 = bf16, 1 = fp32), contiguous, at any element offset.  kahan_comps (the array, or any entry) may be NULL:
+ * no Kahan compensation for that tensor; a non-NULL c needs bf16.  With t the step count, on the host in double and
+ * rounded to fp32: debias(b, t) = (b^t - b) / (b^t - 1), beta1_comp = 1 - debias(beta1, t), beta2_hat = debias(beta2, t),
+ * one_minus_beta2_hat = 1 - beta2_hat, decay = 1 - lr * weight_decay (fully decoupled: 1 - lr / max_lr * weight_decay).
+ *   p *= decay;  m = lerp(m, g, beta1_comp);  v = v * beta2_hat + one_minus_beta2_hat * g * g;
+ *   u = -lr * m / (sqrt(v) + eps);  with c: c += u; old = p; p += c; c += old - p   without: p += u
+ * Each operation is IEEE round-to-nearest fp32 in this order (no FMA), rounded to bf16 where a bf16 torch op rounds;
+ * elementwise, so bitwise repeatable.  Up to 64 tensors per launch.
+ * replaces: optimi.AdamW (Kahan summation for bf16 weights) built for `type = 'adamw_optimi'` (train.py:676-678). */
+int dpipe_adamw_step(void* const* params, const void* const* grads, void* const* exp_avgs, void* const* exp_avg_sqs,
+                     void* const* kahan_comps, const int64_t* numels, const int* dtypes, int n, float lr, float beta1_comp,
+                     float beta2_hat, float one_minus_beta2_hat, float eps, float decay, void* stream);
 /* flow-matching noising of one batch on the device, fp32, IEEE-rounded multiplies and adds (bit-identical to the host ops):
  *   xt = (1 - t[b]) * x1 + t[b] * x0,   target = x0 - x1      x1, x0: [bs, c, frames, h, w] contiguous; t: [bs]
  * pack != 0 (frames == 1): both outputs in diffusers' packed layout [bs, (h/2)(w/2), 4c] (2x2 patches, channel-major).
