@@ -124,6 +124,9 @@ SIGNATURES['dpipe_grad_sumsq'] = (c_int, [c_void_p, c_void_p, c_void_p, c_int, c
 SIGNATURES['dpipe_grad_scale'] = (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p])
 SIGNATURES['dpipe_adamw_step'] = (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float,
                                           c_float, c_float, c_float, c_float, c_float, c_void_p])
+SIGNATURES['dpipe_automagic_scratch_doubles'] = (c_int, [c_void_p, c_int, ctypes.POINTER(c_int64)])
+SIGNATURES['dpipe_automagic_stats'] = (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p])
+SIGNATURES['dpipe_automagic_apply'] = (c_int, [c_void_p, c_int, c_void_p, c_void_p])
 SIGNATURES['dpipe_noise_pack'] = (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int64, c_int, c_int,
                                           c_int, c_void_p])
 SIGNATURES['dpipe_exec_create'] = (c_int, [c_int, c_int, ctypes.c_double, ctypes.POINTER(c_void_p)])
@@ -136,3 +139,16 @@ SIGNATURES['dpipe_exec_load_plan'] = (c_int, [c_void_p, c_void_p, c_int, c_int, 
 SIGNATURES['dpipe_exec_stage_send'] = (c_int, [c_void_p, c_int, c_int, c_int, c_void_p])
 SIGNATURES['dpipe_exec_recv_base'] = (c_int, [c_void_p, c_int, c_int, ctypes.POINTER(c_void_p)])
 SIGNATURES['dpipe_exec_next'] = (c_int, [c_void_p, c_void_p, c_void_p])
+
+
+class AutomagicTensor(ctypes.Structure):
+    _fields_ = [('p', c_void_p), ('g', c_void_p), ('row', c_void_p), ('col', c_void_p), ('v', c_void_p),
+                ('code', c_void_p), ('pol', c_void_p), ('shift', c_void_p), ('scale', c_void_p), ('avg_lr', c_void_p),
+                ('ws', c_void_p), ('numel', c_int64), ('L', c_int64), ('R', c_int64), ('C', c_int64),
+                ('dtype', c_int), ('flags', c_int)]
+
+
+class AutomagicScalars(ctypes.Structure):
+    _fields_ = [('beta2', ctypes.c_double), ('eps', ctypes.c_double), ('lr_bump', ctypes.c_double),
+                ('min_lr', ctypes.c_double), ('max_lr', ctypes.c_double), ('clip_threshold', ctypes.c_double),
+                ('weight_decay', ctypes.c_double)]

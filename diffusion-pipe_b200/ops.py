@@ -4,7 +4,7 @@ import ctypes
 
 import torch
 
-from . import _lib
+from . import _abi, _lib
 from ._abi import AttnArgs, AttnBwdArgs, QkBwdArgs, WanNormBwdArgs, WanNormFwdArgs
 from ._lib import GemmArgs, QkvEpilogue, check, lib
 
@@ -578,6 +578,110 @@ def adamw_step(params, grads, exp_avgs, exp_avg_sqs, kahan_comps, *, lr, beta1_c
           'dpipe_adamw_step')
     _prof_end(_e, 0.0, 'adamw_step')
     LAUNCHES += (n + 63) // 64
+
+
+def automagic_dims(shape):
+    """(factored, L, R, C) of a parameter shape: ndim >= 2 is factored over [L = prod(shape[:-2]), R, C]"""
+    if len(shape) < 2:
+        return False, 1, 1, 1
+    lead = 1
+    for s in shape[:-2]:
+        lead *= int(s)
+    return True, lead, int(shape[-2]), int(shape[-1])
+
+
+def automagic_workspace(params):
+    """one fp32 buffer on the params' device, returned as per-tensor views: [clip divisor, max |new_lr|, avg_lr,
+    fp32(previous scale)] and, for factored tensors, L row means, L*R row factors, L*C column factors (include/dpipe.h)"""
+    sizes = []
+    for p in params:
+        f, L, R, C = automagic_dims(p.shape)
+        sizes.append(4 + (L + L * R + L * C if f else 0))
+    flat = torch.empty(max(1, sum(sizes)), dtype=torch.float32, device=params[0].device if params else 'cpu')
+    return list(torch.split(flat[:sum(sizes)], sizes)) if params else []
+
+
+def _automagic_args(name, params, grads, rows, cols, vs, codes, scales, polarities, shifts, avg_lrs, ws, round_bf16,
+                    beta2, eps, lr_bump, min_lr, max_lr, clip_threshold, weight_decay):
+    n = len(params)
+    lists = (grads, rows, cols, vs, codes, scales, polarities, shifts, avg_lrs, ws, round_bf16)
+    if any(len(x) != n for x in lists):
+        raise ValueError(f'{name}: the tensor lists differ in length')
+    arr = (_abi.AutomagicTensor * max(1, n))()
+
+    def need(t, what, i, dtype, numel):
+        if t is None or not t.is_cuda or t.dtype != dtype or t.numel() != numel or not t.is_contiguous():
+            got = 'None' if t is None else f'{t.dtype} {tuple(t.shape)} on {t.device}'
+            raise TypeError(f'{name}: {what} {i} must be a contiguous CUDA {dtype} tensor of {numel} elements, got {got}')
+        return t.data_ptr()
+    for i, p in enumerate(params):
+        if p.dtype not in _GRAD_DTYPES:
+            raise TypeError(f'{name}: tensor {i} is {p.dtype}; the kernels take bf16 or fp32 weights')
+        f, L, R, C = automagic_dims(p.shape)
+        n_el = p.numel()
+        a = arr[i]
+        a.p = need(p, 'param', i, p.dtype, n_el)
+        a.g = need(grads[i], 'grad', i, p.dtype, n_el)
+        if f:
+            a.row = need(rows[i], 'exp_avg_sq_row', i, torch.float32, L * R)
+            a.col = need(cols[i], 'exp_avg_sq_col', i, torch.float32, L * C)
+        else:
+            a.v = need(vs[i], 'exp_avg_sq', i, torch.float32, n_el)
+        a.code = need(codes[i], 'lr codes', i, torch.int8, n_el)
+        a.pol = need(polarities[i], 'last_polarity', i, torch.bool, n_el)
+        if p.dtype == torch.bfloat16:
+            a.shift = need(shifts[i], 'shift', i, torch.bfloat16, n_el)
+        elif shifts[i] is not None:
+            raise TypeError(f'{name}: tensor {i}: the Kahan shift is for bf16 weights only')
+        a.scale = need(scales[i], 'lr code scale', i, torch.float64, 1)
+        a.avg_lr = need(avg_lrs[i], 'avg_lr', i, torch.float32, 1)
+        a.ws = need(ws[i], 'workspace', i, torch.float32, 4 + (L + L * R + L * C if f else 0))
+        a.numel, a.L, a.R, a.C = n_el, L, R, C
+        a.dtype = _GRAD_DTYPES[p.dtype]
+        a.flags = (1 if f else 0) | (2 if round_bf16[i] else 0)
+    sc = _abi.AutomagicScalars(beta2, eps, lr_bump, min_lr, max_lr, clip_threshold, weight_decay)
+    return arr, n, sc
+
+
+def automagic_stats(params, grads, rows, cols, vs, codes, scales, polarities, shifts, avg_lrs, ws, round_bf16, *, beta2,
+                    eps, lr_bump, min_lr, max_lr, clip_threshold, weight_decay):
+    """Automagic statistics phase (include/dpipe.h dpipe_automagic_stats) over parameter i with its state: rows / cols
+    (factored) or vs (1-D / 0-D) fp32 EMA statistics, updated in place; int8 lr codes, bool last polarity, fp64 0-dim
+    code scale (replaced by the new scale), fp32 0-dim avg_lr (written); ws[i] from automagic_workspace (written);
+    round_bf16[i] for step 1 of a bf16 parameter.  No host synchronisation."""
+    global LAUNCHES
+    arr, n, sc = _automagic_args('automagic_stats', params, grads, rows, cols, vs, codes, scales, polarities, shifts,
+                                 avg_lrs, ws, round_bf16, beta2, eps, lr_bump, min_lr, max_lr, clip_threshold, weight_decay)
+    if n == 0:
+        return
+    need = ctypes.c_int64()
+    check(lib().dpipe_automagic_scratch_doubles(arr, n, ctypes.byref(need)), 'dpipe_automagic_scratch_doubles')
+    scratch = torch.empty(max(1, need.value), dtype=torch.float64, device=params[0].device)
+    _e = _prof_begin()
+    check(lib().dpipe_automagic_stats(arr, n, ctypes.byref(sc), scratch.data_ptr(), scratch.numel(), _stream()),
+          'dpipe_automagic_stats')
+    _prof_end(_e, 0.0, 'automagic_stats')
+    LAUNCHES += 5 * ((n + 63) // 64)
+
+
+def automagic_apply(params, grads, rows, cols, vs, codes, scales, polarities, shifts, avg_lrs, ws, round_bf16, *, beta2,
+                    eps, lr_bump, min_lr, max_lr, clip_threshold, weight_decay):
+    """Automagic apply phase (include/dpipe.h dpipe_automagic_apply) after automagic_stats on the same arguments: new
+    polarity and lr codes, weight decay, Kahan-summed bf16 (plain fp32) weight update, in place; the weights' version
+    counters move."""
+    global LAUNCHES
+    arr, n, sc = _automagic_args('automagic_apply', params, grads, rows, cols, vs, codes, scales, polarities, shifts,
+                                 avg_lrs, ws, round_bf16, beta2, eps, lr_bump, min_lr, max_lr, clip_threshold, weight_decay)
+    if n == 0:
+        return
+    _e = _prof_begin()
+    check(lib().dpipe_automagic_apply(arr, n, ctypes.byref(sc), _stream()), 'dpipe_automagic_apply')
+    _prof_end(_e, 0.0, 'automagic_apply')
+    LAUNCHES += (n + 63) // 64
+    # the kernel wrote the weights behind autograd's back: move their version counters as an in-place op would, so
+    # that caches keyed on them (lora.py's fused factor buffers) see the new values
+    for p in params:
+        torch.autograd.graph.increment_version(p)
 
 
 def noise_pack(x1, x0, t, pack):

@@ -94,3 +94,180 @@ class AdamW(torch.optim.Optimizer):
                 ops.adamw_step(ps, [p.grad for p in ps], [s['exp_avg'] for s in st], [s['exp_avg_sq'] for s in st],
                                [s.get('kahan_comp') for s in st], **sc)
         return loss
+
+
+_AUTOMAGIC_STATS = ('exp_avg_sq_row', 'exp_avg_sq_col', 'exp_avg_sq')
+
+
+class Automagic(torch.optim.Optimizer):
+    """The reference's Automagic (optimizers/automagic.py, `type = 'automagic'`): a per-element learning rate that grows
+    by lr_bump while the sign of the update holds and shrinks when it flips, on Adafactor-style factored second moments,
+    with Kahan-summed bf16 weights.  Each step is two fused phases per param group (`ops.automagic_stats`, then
+    `ops.automagic_apply`; csrc/automagic.cu), with no host synchronisation.
+
+    As in the reference: a start lr above 1e-3 is replaced by 1e-6 (with a warning) for the mask, `group['lr']` keeps the
+    given value and nothing in the step reads it, so LR schedulers have no effect; lr_bump, min_lr and max_lr apply to the
+    whole optimizer, beta2, eps, clip_threshold and weight_decay per group.  Parameters without a gradient are skipped
+    and their step count does not advance.
+
+    State per parameter: `step` (host int); `exp_avg_sq_row` / `exp_avg_sq_col` (factored, ndim >= 2) or `exp_avg_sq`,
+    fp32 (at step 1 of a bf16 parameter they hold the bf16-rounded values the reference's bf16 state holds); the
+    lr mask as int8 codes `lr_mask_q` with an fp64 0-dim `lr_mask_scale`; `last_polarity` (bool); `shift` (bf16 weights
+    only); `avg_lr` (fp32 0-dim).  4 B per bf16 parameter plus the factored vectors (adamw_optimi: 6 B).  The reference's
+    `RMS` entry (the weights' RMS, written and never read) is not kept.  state_dict() writes the lr mask in the
+    reference's format {'quantized', 'scale', 'orig_dtype'} (one sync per tensor, at save time only), and
+    load_state_dict() reads it, including a state dict written by the reference; one without any `lr_mask` is ignored,
+    as in the reference.  Parameters must be bf16 / fp32 tensors (fp16 and fp8 are refused here) on a CUDA device: the
+step kernels refuse CPU tensors, there is no CPU path."""
+
+    def __init__(self, params, lr=1e-6, min_lr=1e-7, max_lr=1e-3, lr_bump=1e-6, eps=(1e-30, 1e-3), clip_threshold=1.0,
+                 beta2=0.999, weight_decay=0.0, do_paramiter_swapping=False, paramiter_swapping_factor=0.1):
+        if do_paramiter_swapping:
+            raise NotImplementedError('automagic: do_paramiter_swapping is not supported (every parameter with a '
+                                      'gradient steps)')
+        self.lr = lr
+        if self.lr > 1e-3:
+            print(f'Warning! Start lr is very high: {self.lr}. Forcing to 1e-6. this does not work like prodigy')
+            self.lr = 1e-6
+        self.min_lr, self.max_lr, self.lr_bump = min_lr, max_lr, lr_bump
+        defaults = dict(lr=lr, eps=eps, clip_threshold=clip_threshold, beta2=beta2, weight_decay=weight_decay)
+        super().__init__(params, defaults)
+        self.base_lrs = [lr for _ in self.param_groups]
+        for group in self.param_groups:
+            for p in group['params']:
+                if p.dtype not in (torch.bfloat16, torch.float32):
+                    raise TypeError(f'automagic: parameters must be bf16 or fp32 tensors, got {p.dtype}')
+
+    def _mask_init(self, p):
+        """codes and scale of the constant start mask, quantized on the host exactly as on CPU (no device sync)"""
+        amax = _f32(self.lr)
+        scale = amax / 127.0 if amax > 0 else 1.0
+        q = torch.round(torch.tensor(amax, dtype=torch.float32) / torch.tensor(scale, dtype=torch.float32))
+        q = int(q.clamp(-127, 127))
+        return q, scale
+
+    def _init_state(self, p):
+        state = self.state[p]
+        q, scale = self._mask_init(p)
+        dev = p.device
+        state['step'] = 0
+        state['lr_mask_q'] = torch.full(p.shape, q, dtype=torch.int8, device=dev)
+        state['lr_mask_scale'] = torch.full((), scale, dtype=torch.float64, device=dev)      # a fill: no host copy
+        state['avg_lr'] = torch.full((), _f32(q * _f32(scale)), dtype=torch.float32, device=dev)
+        state['last_polarity'] = torch.zeros(p.shape, dtype=torch.bool, device=dev)
+        if p.ndim >= 2:
+            state['exp_avg_sq_row'] = torch.zeros(p.shape[:-1], dtype=torch.float32, device=dev)
+            state['exp_avg_sq_col'] = torch.zeros(p.shape[:-2] + p.shape[-1:], dtype=torch.float32, device=dev)
+        else:
+            state['exp_avg_sq'] = torch.zeros(p.shape, dtype=torch.float32, device=dev)
+        if p.dtype == torch.bfloat16:
+            state['shift'] = torch.zeros_like(p, memory_format=torch.contiguous_format)
+        return state
+
+    @staticmethod
+    def _get_lr(state):
+        return state['avg_lr'] if 'avg_lr' in state else 0.0
+
+    def _get_group_lr(self, group):
+        lrs = [self._get_lr(self.state[p]) for p in group['params']]
+        if not lrs:
+            return self.lr
+        return float(sum(lrs) / len(lrs))
+
+    def get_learning_rates(self):
+        """the mean avg_lr of each group's parameters (logging only: reads device scalars)"""
+        lrs = [self._get_group_lr(group) for group in self.param_groups]
+        return lrs if lrs else self.base_lrs
+
+    def get_avg_learning_rate(self):
+        lrs = self.get_learning_rates()
+        return sum(lrs) / len(lrs)
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        for group in self.param_groups:
+            ps = [p for p in group['params'] if p.grad is not None and p.requires_grad]
+            if not ps:
+                continue
+            sts = []
+            for p in ps:
+                st = self.state[p] if self.state[p] else self._init_state(p)
+                st['step'] += 1
+                sts.append(st)
+            eps = group['eps']
+            if isinstance(eps, (tuple, list)):
+                eps = eps[0]
+            args = ([p.grad for p in ps], [s.get('exp_avg_sq_row') for s in sts], [s.get('exp_avg_sq_col') for s in sts],
+                    [s.get('exp_avg_sq') for s in sts], [s['lr_mask_q'] for s in sts], [s['lr_mask_scale'] for s in sts],
+                    [s['last_polarity'] for s in sts], [s.get('shift') for s in sts], [s['avg_lr'] for s in sts],
+                    ops.automagic_workspace(ps),
+                    [p.dtype == torch.bfloat16 and s['step'] == 1 for p, s in zip(ps, sts)])
+            sc = dict(beta2=group['beta2'], eps=eps, lr_bump=self.lr_bump, min_lr=self.min_lr, max_lr=self.max_lr,
+                      clip_threshold=group['clip_threshold'], weight_decay=group['weight_decay'])
+            ops.automagic_stats(ps, *args, **sc)
+            ops.automagic_apply(ps, *args, **sc)
+        return loss
+
+    def state_dict(self):
+        sd = super().state_dict()
+        out = {}
+        for k, st in sd['state'].items():
+            s = {kk: v for kk, v in st.items() if kk not in ('lr_mask_q', 'lr_mask_scale')}
+            if 'lr_mask_q' in st:
+                s['lr_mask'] = {'quantized': st['lr_mask_q'], 'scale': float(st['lr_mask_scale'].item()),
+                                'orig_dtype': torch.float32}
+            out[k] = s
+        sd['state'] = out
+        return sd
+
+    def load_state_dict(self, state_dict):
+        saved = state_dict.get('state') if isinstance(state_dict, dict) else None
+        if not isinstance(saved, dict) or not any(isinstance(s, dict) and 'lr_mask' in s for s in saved.values()):
+            return                      # not an Automagic state: ignored, as in the reference
+        groups, saved_groups = self.param_groups, state_dict['param_groups']
+        if len(groups) != len(saved_groups) or any(len(g['params']) != len(s['params'])
+                                                    for g, s in zip(groups, saved_groups)):
+            raise ValueError('automagic: the loaded state dict has a different parameter group layout')
+        for g, s in zip(groups, saved_groups):
+            for k, v in s.items():
+                if k != 'params':
+                    g[k] = v
+        self.state.clear()
+        for g, s in zip(groups, saved_groups):
+            for p, pid in zip(g['params'], s['params']):
+                if pid in saved:
+                    self.state[p] = self._state_from_saved(p, saved[pid])
+
+    def _state_from_saved(self, p, s):
+        """a saved (or reference) per-parameter state on p's device; statistics as fp32 (the reference's are bf16 after
+        step 1 of a bf16 parameter), keeping their precision; copies, never views of the saved tensors"""
+        dev = p.device
+        st = {'step': int(s.get('step', 0))}
+        if 'lr_mask' in s:
+            m = s['lr_mask']
+            st['lr_mask_q'] = m['quantized'].to(device=dev, dtype=torch.int8).clone(memory_format=torch.contiguous_format)
+            st['lr_mask_scale'] = torch.tensor(float(m['scale']), dtype=torch.float64, device=dev)
+        else:
+            q, scale = self._mask_init(p)
+            st['lr_mask_q'] = torch.full(p.shape, q, dtype=torch.int8, device=dev)
+            st['lr_mask_scale'] = torch.tensor(scale, dtype=torch.float64, device=dev)
+        avg = s.get('avg_lr', 0.0)
+        st['avg_lr'] = torch.as_tensor(avg, dtype=torch.float32).to(dev).reshape(())
+        pol = s.get('last_polarity')
+        st['last_polarity'] = (pol.to(device=dev, dtype=torch.bool).clone(memory_format=torch.contiguous_format) if pol is not None else
+                               torch.zeros(p.shape, dtype=torch.bool, device=dev))
+        if p.ndim >= 2:
+            for k, shape in (('exp_avg_sq_row', p.shape[:-1]), ('exp_avg_sq_col', p.shape[:-2] + p.shape[-1:])):
+                st[k] = (s[k].to(device=dev, dtype=torch.float32).clone(memory_format=torch.contiguous_format) if k in s else
+                         torch.zeros(shape, dtype=torch.float32, device=dev))
+        else:
+            st['exp_avg_sq'] = (s['exp_avg_sq'].to(device=dev, dtype=torch.float32).clone(memory_format=torch.contiguous_format) if 'exp_avg_sq' in s
+                                else torch.zeros(p.shape, dtype=torch.float32, device=dev))
+        if p.dtype == torch.bfloat16:
+            st['shift'] = (s['shift'].to(device=dev, dtype=torch.bfloat16).clone(memory_format=torch.contiguous_format) if 'shift' in s else
+                           torch.zeros_like(p, memory_format=torch.contiguous_format))
+        return st

@@ -258,6 +258,61 @@ int dpipe_grad_scale(const void* const* ptrs, const int64_t* numels, const int* 
 int dpipe_adamw_step(void* const* params, const void* const* grads, void* const* exp_avgs, void* const* exp_avg_sqs,
                      void* const* kahan_comps, const int64_t* numels, const int* dtypes, int n, float lr, float beta1_comp,
                      float beta2_hat, float one_minus_beta2_hat, float eps, float decay, void* stream);
+/* One parameter of an Automagic step (the reference's optimizers/automagic.py).  All tensors contiguous, at any element
+ * offset.  p / g / shift: dtype (0 = bf16, 1 = fp32), numel elements; shift (Kahan) for bf16 weights only, NULL for fp32.
+ * flags & DPIPE_AUTOMAGIC_FACTORED (ndim >= 2): shape = [L (= prod(shape[:-2]), 1 for 2-D), R, C], row = exp_avg_sq_row
+ * [L*R] and col = exp_avg_sq_col [L*C] fp32; otherwise v = exp_avg_sq [numel] fp32.  flags & DPIPE_AUTOMAGIC_ROUND_BF16:
+ * step 1 of a bf16 parameter, where the reference's statistics are bf16 tensors: every op on them and on u rounds to bf16.
+ * code: int8 lr codes, pol: last polarity (bool bytes), scale: the codes' scale (fp64 scalar), avg_lr: fp32 scalar.
+ * ws (fp32, per tensor, written by dpipe_automagic_stats, read by dpipe_automagic_apply):
+ *   ws[0] clip divisor max(rms(u) / clip_threshold, 1)   ws[1] max |new_lr|   ws[2] avg_lr   ws[3] fp32(previous scale)
+ *   factored only: ws[4 .. 4+L) row.mean(-1), then L*R row factors rsqrt(row / row.mean(-1)), then L*C column factors
+ *   rsqrt(col): 4 + L + L*R + L*C floats; unfactored: 4 floats. */
+#define DPIPE_AUTOMAGIC_FACTORED 1
+#define DPIPE_AUTOMAGIC_ROUND_BF16 2
+typedef struct dpipe_automagic_tensor {
+    void* p;
+    const void* g;
+    float* row;
+    float* col;
+    float* v;
+    signed char* code;
+    unsigned char* pol;
+    void* shift;
+    double* scale;
+    float* avg_lr;
+    float* ws;
+    int64_t numel, L, R, C;
+    int dtype;
+    int flags;
+} dpipe_automagic_tensor;
+/* the group's hyper-parameters, as the Python floats the reference passes; the kernels use their fp32 roundings
+ * (alpha = fp32(1 - beta2), -weight_decay), and eps is eps[0] of the reference's tuple */
+typedef struct dpipe_automagic_scalars {
+    double beta2, eps, lr_bump, min_lr, max_lr, clip_threshold, weight_decay;
+} dpipe_automagic_scalars;
+/* doubles of fp64 scratch dpipe_automagic_stats needs for these tensors (row / column partials and per-CTA sums of
+ * the largest chunk of 64) */
+int dpipe_automagic_scratch_doubles(const dpipe_automagic_tensor* t, int n, int64_t* out);
+/* Automagic statistics phase over n parameters, up to 64 per launch group (5 launches per group, none per tensor):
+ *   u0 = g*g + eps;  factored: row = EMA_beta2(u0.mean(-1)), col = EMA_beta2(u0.mean(-2)),
+ *                    u = (rsqrt(row / row.mean(-1)) * rsqrt(col)) * g;   unfactored: v = EMA_beta2(u0), u = rsqrt(v) * g
+ *   (EMA: x = x * beta2 + (1 - beta2) * mean, torch's fused add with alpha)
+ *   new_lr = clamp(q * scale +- lr_bump, min_lr, max_lr), + where (u > 0) == last polarity
+ *   clip divisor = max(fp32(sqrt(sum u^2)) / fp32(sqrt(numel)) / clip_threshold, 1); avg_lr = mean(new_lr);
+ *   scale = max|new_lr| / 127 (fp64; 1 when 0).  Row means, factors and the per-tensor scalars go to ws (above).
+ * Reductions accumulate in fp64 in a fixed order (bitwise repeatable), no float atomics, no host synchronisation.
+ * replaces: the statistics half of Automagic.step (optimizers/automagic.py:240-300, optimizer_utils.py:222-232). */
+int dpipe_automagic_stats(const dpipe_automagic_tensor* t, int n, const dpipe_automagic_scalars* s, double* scratch,
+                          int64_t scratch_len, void* stream);
+/* Automagic apply phase, one launch per group of 64, after dpipe_automagic_stats on the same tensors: u as above,
+ * u /= clip divisor, new polarity, codes = clamp(round(new_lr / fp32(scale)), -127, 127), u *= new_lr, then
+ *   bf16: upd = -u + p * (-weight_decay) * new_lr; shift += upd; old = p; p += shift; shift += old - p
+ *   fp32: p += p * (-weight_decay) * new_lr; p -= u            (the weight-decay term only when weight_decay != 0)
+ * Each operation is IEEE round-to-nearest fp32 in the reference's op order (no FMA), rounded to bf16 where a bf16
+ * torch op rounds: bit-identical to oracle/automagic_ref.py automagic_apply_emulated.
+ * replaces: the update half of Automagic.step (optimizers/automagic.py:300-344). */
+int dpipe_automagic_apply(const dpipe_automagic_tensor* t, int n, const dpipe_automagic_scalars* s, void* stream);
 /* flow-matching noising of one batch on the device, fp32, IEEE-rounded multiplies and adds (bit-identical to the host ops):
  *   xt = (1 - t[b]) * x1 + t[b] * x0,   target = x0 - x1      x1, x0: [bs, c, frames, h, w] contiguous; t: [bs]
  * pack != 0 (frames == 1): both outputs in diffusers' packed layout [bs, (h/2)(w/2), 4c] (2x2 patches, channel-major).

@@ -6,8 +6,9 @@
 Same CLI flags and TOML keys as the reference for everything on the hot path (SURVEY.md Appendix B): the model table,
 `pipeline_stages`, `micro_batch_size_per_gpu` (int or [[res, bs], ...]), `gradient_accumulation_steps`,
 `gradient_clipping`, `partition_method` / `partition_split`, `[optimizer]` (type adamw = torch's fused AdamW, adamw_optimi =
-optimi's AdamW with Kahan-summed bf16 weights on the fused step kernel, sgd; `betas`, `weight_decay`, `eps`, `lr`,
-`kahan_sum`, `decouple_lr`, `max_lr`), `lr_scheduler`, `warmup_steps`, `epochs`, `max_steps`, `save_every_n_*`,
+optimi's AdamW with Kahan-summed bf16 weights on the fused step kernel, automagic = the reference's Automagic on its
+fused step kernels, sgd; `betas`, `weight_decay`, `eps`, `lr`, `kahan_sum`, `decouple_lr`, `max_lr`; automagic:
+`min_lr`, `max_lr`, `lr_bump`, `clip_threshold`, `beta2`), `lr_scheduler`, `warmup_steps`, `epochs`, `max_steps`, `save_every_n_*`,
 `checkpoint_every_n_minutes`, `--resume_from_checkpoint`, `--reset_dataloader`, `--reset_optimizer`.
 
 What is deliberately NOT here (out of the hot path, SURVEY.md section 8): VAE / text-encoder caching of a raw image
@@ -262,6 +263,9 @@ def make_optimizer_factory(config, model, global_batch_size=1):
         if typ == 'adamw_optimi':                       # optimi.AdamW (train.py:676-678): Kahan-summed bf16 weights, optimi's defaults
             from diffusion_pipe_b200 import optim
             return optim.AdamW(groups, **oc)
+        if typ == 'automagic':                          # optimizers/automagic.py (train.py:692-694): fused step kernels
+            from diffusion_pipe_b200 import optim
+            return optim.Automagic(groups, **oc)
         if typ == 'sgd':
             return torch.optim.SGD(groups, **oc)
         raise NotImplementedError(f'optimizer type {typ} is not wired into this driver (third-party optimizers are out of '
