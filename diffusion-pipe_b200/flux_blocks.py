@@ -9,12 +9,19 @@ Parameter names follow diffusers' FluxTransformerBlock / FluxSingleTransformerBl
 at models/flux.py:490-533), so `p.original_name`, checkpoints and optimizers see the same model.  Projections that the
 kernels consume as one matrix (q,k,v[,proj_mlp]) are allocated fused and exposed through per-projection *views*.
 
+**GEMM sites.**  The block functions never touch a linear's weight directly: they read the block's `sites`, one object
+per GEMM (`DenseSite` here, `lora.LoraSite` once adapters are attached) and one per modulation linear (`DenseMod` /
+`lora.ModLora`).  A dense site is the LoRA site's interface with R = 0 adapter columns: the same operands, buffers and
+weight-gradient queueing, so one function serves dense and LoRA training and the two never drift apart.  The sites
+also hold the policy for the LayerNorm+modulation outputs that feed a GEMM (`keep` / `rebuild`, see DESIGN.md §3).
+
 The arithmetic (including where bf16 roundings happen under the reference's autocast) is the one restated in
 oracle/flux_ref.py; tests/test_flux_blocks_gpu.py checks both directions against it.
 
-Memory policy (H100, 80 GB): no activation recompute at all — a block saves its bf16 intermediates, including the
+Memory policy (H100, 80 GB): dense training recomputes nothing — a block saves its bf16 intermediates, including the
 LayerNorm+modulation outputs that feed its GEMMs (~0.54 GB per block per sample at 1024^2; round 1 recomputed those two
-HBM passes per stream in backward: 1.5 % of the step for 2 GB per sample).
+HBM passes per stream in backward: 1.5 % of the step for 2 GB per sample).  With adapters only their R columns are
+kept and the LayerNorm is recomputed in backward (lora.py).
 """
 import torch
 from torch import nn
@@ -109,11 +116,111 @@ def _acc_vec(p, g32):
         p.grad.add_(g32.view_as(p))
 
 
-def _acc_fused_bias(fp, bgrad, acc, g32):
-    if acc:
-        bgrad.add_(g32)
-    else:
-        bgrad.copy_(g32)
+def _defer_acc(*pairs):
+    """queues p.grad (+)= g32 for the (vector parameter, fp32 gradient) pairs whose parameter is trained"""
+    pairs = [(p, g) for p, g in pairs if p.requires_grad]
+    if pairs:
+        ops.defer(lambda: [_acc_vec(p, g) for p, g in pairs])
+
+
+# =====================================================================================================================
+# GEMM sites without an adapter (the R = 0 form of lora.LoraSite)
+# =====================================================================================================================
+class DenseSite:
+    """One GEMM `y = x W^T + b` of a block over a `_Lin` or a `FusedParam`.  Operands are the weight itself, activation
+    buffers are plain `[rows, K]` / `[rows, N]`, and the weight gradient dW (+)= dy^T x plus the bias gradient are queued
+    when the weight is trained."""
+    R = 0
+
+    def __init__(self, lin):
+        self.lin = lin
+
+    @property
+    def w_fwd(self):
+        return self.lin.weight
+
+    w_dgrad = w_fwd
+
+    @property
+    def bias(self):
+        return self.lin.bias
+
+    @property
+    def K(self):
+        return self.lin.weight.shape[1]
+
+    @property
+    def N(self):
+        return self.lin.weight.shape[0]
+
+    @property
+    def bias_grad(self):
+        """True when queue_grads also needs the fp32 bias gradient (i.e. the site's weight is trained)"""
+        lin = self.lin
+        return lin.requires_grad() if isinstance(lin, FusedParam) else lin.weight.requires_grad
+
+    def refresh(self):
+        pass
+
+    def alloc_in(self, rows, device):
+        return torch.empty((rows, self.K), dtype=torch.bfloat16, device=device)
+
+    def alloc_dy(self, rows, device, spare=None):
+        """[rows, N] dy buffer; `spare`, a dead [rows, N] buffer of the caller, is used instead of a new one"""
+        return torch.empty((rows, self.N), dtype=torch.bfloat16, device=device) if spare is None else spare
+
+    def input_operand(self, x):
+        return x
+
+    def project(self, xa):
+        pass
+
+    def backproject(self, dya):
+        pass
+
+    def keep(self, xa, recompute=False):
+        """what backward keeps of the LayerNorm output `xa` feeding this site: the buffer itself, or nothing when the
+        caller recomputes it (Wan: its storage is recycled in forward)"""
+        return None if recompute else xa
+
+    def spare(self, xa):
+        """xa's storage for the caller to reuse as a [rows, K] output once xa is dead"""
+        return xa
+
+    def rebuild(self, kept, rows, device, ln):
+        """the input operand again in backward; `ln(out)` recomputes the LayerNorm into `out`"""
+        if kept is not None:
+            return kept
+        xa = self.alloc_in(rows, device)
+        ln(xa)
+        return xa
+
+    def dgrad_out(self, xa):
+        """output buffer of the input-gradient GEMM: xa's storage, unless a deferred weight gradient still reads xa"""
+        return None if ops.deferring() else xa
+
+    def queue_grads(self, x, dy, db=None):
+        """dW (+)= dy^T x and b (+)= db as deferred weight-gradient work.  x, dy may be lists of row blocks (one per
+        sample): their products are accumulated into one gradient and the bias is added once."""
+        if not self.bias_grad:
+            return
+        xs, dys = (x, dy) if isinstance(x, list) else ([x], [dy])
+
+        def wgrad(lin=self.lin, xs=xs, dys=dys, db=db):
+            fused = isinstance(lin, FusedParam)
+            if fused:
+                g, bg, acc = lin.grads()
+            else:
+                g, acc = _grad_buf(lin.weight)
+            for i, (x, dy) in enumerate(zip(xs, dys)):
+                ops.gemm(dy, x, a_mn=True, b_mn=True, out=g, accumulate=acc or i > 0)
+            if not fused:
+                _acc_vec(lin.bias, db)
+            elif acc:
+                bg.add_(db)
+            else:
+                bg.copy_(db)
+        ops.defer(wgrad)
 
 
 # =====================================================================================================================
@@ -134,6 +241,27 @@ def _mod_bwd(dmod32, temb, lin, d_temb32):
         _acc_vec(lin.bias, dbias)
 
 
+class DenseMod:
+    """modulation linear without an adapter (the interface of lora.ModLora)"""
+
+    def __init__(self, lin):
+        self.lin = lin
+
+    def refresh(self):
+        pass
+
+    def fwd(self, temb):
+        return _mod_fwd(temb, self.lin), None
+
+    def bwd(self, dmod32, temb, saved, d_temb32):
+        _mod_bwd(dmod32, temb, self.lin, d_temb32)
+
+
+def _refresh(sites):
+    for s in sites.values():
+        s.refresh()
+
+
 # =====================================================================================================================
 # double-stream block
 # =====================================================================================================================
@@ -142,14 +270,15 @@ def _valid_rows(n_txt, Lt, Ltot, device):
     return torch.cat([torch.arange(n_txt, device=device), torch.arange(Lt, Ltot, device=device)])
 
 
-def _ragged_attn_fwd(q, k, v, Lt, txt_lens):
+def _ragged_attn_fwd(q, k, v, Lt, txt_lens, out):
     """Joint attention for a micro-batch whose prompts have different lengths (key-padding mask of
     models/qwen_image.py:472-476): every sample attends over its own valid rows only — gathered into a dense
-    [1, H, L_b, 128] problem for the same kernels.  Padded text rows are neither keys nor (meaningful) queries; their
-    output is zero, which no loss term can see (they are masked out of the keys of every later block)."""
+    [1, H, L_b, 128] problem for the same kernels — and its output lands in the first H*128 columns of `out`
+    [B*Ltot, >= H*128].  Padded text rows are neither keys nor (meaningful) queries; their output is zero, which no loss
+    term can see (they are masked out of the keys of every later block)."""
     B, H, Ltot, _ = q.shape
-    o = torch.zeros((B * Ltot, H * HD), dtype=q.dtype, device=q.device)
-    o3 = o.view(B, Ltot, H * HD)
+    out[:, :H * HD].zero_()
+    o3 = out.view(B, Ltot, out.shape[1])[:, :, :H * HD]
     saved = []
     for b, n in enumerate(txt_lens):
         idx = _valid_rows(int(n), Lt, Ltot, q.device)
@@ -157,7 +286,7 @@ def _ragged_attn_fwd(q, k, v, Lt, txt_lens):
         ob, lse_b = ops.attn_fwd(qb, kb, vb)
         o3[b].index_copy_(0, idx, ob)
         saved.append((idx, qb, kb, vb, ob, lse_b))
-    return o, saved
+    return saved
 
 
 def _ragged_attn_bwd(saved, d_o, shape):
@@ -174,13 +303,19 @@ def _ragged_attn_bwd(saved, d_o, shape):
 
 class _Stream:
     """Per-stream (image or text) state saved by the double block forward."""
-    __slots__ = ('x', 'mod', 'mean1', 'rstd1', 'xn', 'y_attn', 'x1', 'mean2', 'rstd2', 'xn2', 'u', 'h', 'y_mlp', 'L', 'off')
+    __slots__ = ('x', 'mod', 'mod_saved', 'mean1', 'rstd1', 'xn', 'y_attn', 'x1', 'mean2', 'rstd2', 'xn2', 'u', 'h',
+                 'y_mlp', 'L', 'off')
 
 
 class FluxDoubleBlockFn(torch.autograd.Function):
+    """Flux / Qwen-Image double-stream block over `blk.sites` (keys: mod, mod_c, qkv, add_qkv, to_out, to_add_out, ff1,
+    ff2, ffc1, ffc2; the *_c / add_* / ffc* sites serve the text stream)."""
+
     @staticmethod
     def forward(ctx, blk, hidden, enc, temb, cos, sin, txt_lens=None):
         """txt_lens: None (every text row is a real token) or one prompt length per sample (Qwen-Image key mask)"""
+        S = blk.sites
+        _refresh(S)
         B, Li, D = hidden.shape
         Lt = enc.shape[1]
         Ltot = Li + Lt
@@ -188,56 +323,62 @@ class FluxDoubleBlockFn(torch.autograd.Function):
         dev = hidden.device
         bf = torch.bfloat16
         shp = (B, H, Ltot, HD)
-        q = torch.empty(shp, dtype=bf, device=dev)
-        k = torch.empty(shp, dtype=bf, device=dev)
-        v = torch.empty(shp, dtype=bf, device=dev)
-        qhat = torch.empty(shp, dtype=bf, device=dev)
-        khat = torch.empty(shp, dtype=bf, device=dev)
+        q, k, v, qhat, khat = (torch.empty(shp, dtype=bf, device=dev) for _ in range(5))
         q_rstd = torch.empty((B, H, Ltot), dtype=torch.float32, device=dev)
         k_rstd = torch.empty((B, H, Ltot), dtype=torch.float32, device=dev)
         streams = []
-        # (input, rows, seq offset, modulation linear, fused qkv, q/k norm weights)
-        spec = ((hidden, Li, Lt, blk.norm1.linear, blk.qkv, blk.attn.norm_q, blk.attn.norm_k),
-                (enc, Lt, 0, blk.norm1_context.linear, blk.add_qkv, blk.attn.norm_added_q, blk.attn.norm_added_k))
-        for x3, L, off, modlin, fq, nq, nk in spec:
+        # (input, rows, seq offset, modulation, qkv site, q/k norm weights)
+        spec = ((hidden, Li, Lt, S['mod'], S['qkv'], blk.attn.norm_q, blk.attn.norm_k),
+                (enc, Lt, 0, S['mod_c'], S['add_qkv'], blk.attn.norm_added_q, blk.attn.norm_added_k))
+        for x3, L, off, ml, sq, nq, nk in spec:
             st = _Stream()
             st.L, st.off = L, off
             st.x = x3.reshape(B * L, D)
-            st.mod = _mod_fwd(temb, modlin)                               # [B, 6D]: shift,scale,gate (msa), shift,scale,gate (mlp)
+            st.mod, st.mod_saved = ml.fwd(temb)                             # [B, 6D]: shift,scale,gate (msa), shift,scale,gate (mlp)
             m = st.mod
-            xn, st.mean1, st.rstd1 = ops.ln_modulate_fwd(st.x, m[:, D:2 * D], m[:, 0:D], B, L)
+            xa = sq.alloc_in(B * L, dev)
+            _, st.mean1, st.rstd1 = ops.ln_modulate_fwd(st.x, m[:, D:2 * D], m[:, 0:D], B, L, out=xa[:, :D])
+            sq.project(xa)
             e = ops.make_qkv_epilogue(q, k, v, nq.weight, nk.weight, cos, sin, H, Ltot, off, qhat, khat, q_rstd, k_rstd)
-            ops.gemm(xn, fq.weight, bias=fq.bias, epilogue=ops.EPI_QKV_ROPE, out=xn, rows_per_batch=L, qkv=e)   # (no token-major output: `out` is not written)
-            st.xn = xn
+            ops.gemm(xa, sq.w_fwd, bias=sq.bias, epilogue=ops.EPI_QKV_ROPE, out=xa, rows_per_batch=L, qkv=e)   # (no token-major output: `out` is not written)
+            st.xn = sq.keep(xa)
             streams.append(st)
+        so, sao = S['to_out'], S['to_add_out']
+        assert so.R == sao.R
+        oa = so.alloc_in(B * Ltot, dev)                                     # attention output (+ adapter columns), token-major
         if txt_lens is None:
-            o, lse = ops.attn_fwd(q, k, v)                                # o: [B*Ltot, H*HD] token-major
+            _, lse = ops.attn_fwd(q, k, v, out=oa)
         else:
-            o, lse = _ragged_attn_fwd(q, k, v, Lt, txt_lens)              # lse: per-sample saved state
+            lse = _ragged_attn_fwd(q, k, v, Lt, txt_lens, oa)               # lse: per-sample saved state
         ctx.ragged = txt_lens is not None
-        o3 = o.view(B, Ltot, H * HD)
+        oa3 = oa.view(B, Ltot, oa.shape[1])
         outs = []
-        tail = ((blk.attn.to_out[0], blk.ff), (blk.attn.to_add_out, blk.ff_context))
-        for st, (wo, ff) in zip(streams, tail):
+        tail = ((so, S['ff1'], S['ff2']), (sao, S['ffc1'], S['ffc2']))
+        for st, (swo, s1, s2) in zip(streams, tail):
             L, off, m = st.L, st.off, st.mod
             st.y_attn = torch.empty((B * L, D), dtype=bf, device=dev)
             st.x1 = torch.empty((B * L, D), dtype=bf, device=dev)
-            for b in range(B):                                            # rows of one sample are contiguous in o
+            for b in range(B):                                              # rows of one sample are contiguous in o
                 rs = slice(b * L, (b + 1) * L)
-                ops.gemm(o3[b, off:off + L], wo.weight, bias=wo.bias, epilogue=ops.EPI_GATE_RES, aux=st.x[rs],
+                rows = oa3[b, off:off + L]
+                swo.project(rows)
+                ops.gemm(rows, swo.w_fwd, bias=swo.bias, epilogue=ops.EPI_GATE_RES, aux=st.x[rs],
                          gate=m[b:b + 1, 2 * D:3 * D], out=st.x1[rs], out2=st.y_attn[rs], rows_per_batch=L)
-            xn2, st.mean2, st.rstd2 = ops.ln_modulate_fwd(st.x1, m[:, 4 * D:5 * D], m[:, 3 * D:4 * D], B, L)
-            st.xn2 = xn2
-            w1, w2 = ff.net[0].proj, ff.net[2]
-            st.u = torch.empty((B * L, w1.weight.shape[0]), dtype=bf, device=dev)
-            st.h = ops.gemm(xn2, w1.weight, bias=w1.bias, epilogue=ops.EPI_BIAS_GELU, out2=st.u)
+            x2a = s1.alloc_in(B * L, dev)
+            _, st.mean2, st.rstd2 = ops.ln_modulate_fwd(st.x1, m[:, 4 * D:5 * D], m[:, 3 * D:4 * D], B, L, out=x2a[:, :D])
+            s1.project(x2a)
+            st.xn2 = s1.keep(x2a)
+            st.u = torch.empty((B * L, s1.N), dtype=bf, device=dev)
+            st.h = s2.alloc_in(B * L, dev)
+            ops.gemm(x2a, s1.w_fwd, bias=s1.bias, epilogue=ops.EPI_BIAS_GELU, out=st.h[:, :s1.N], out2=st.u)
+            s2.project(st.h)
             st.y_mlp = torch.empty((B * L, D), dtype=bf, device=dev)
-            x2 = ops.gemm(st.h, w2.weight, bias=w2.bias, epilogue=ops.EPI_GATE_RES, aux=st.x1,
+            x2 = ops.gemm(st.h, s2.w_fwd, bias=s2.bias, epilogue=ops.EPI_GATE_RES, aux=st.x1,
                           gate=m[:, 5 * D:6 * D], out2=st.y_mlp, rows_per_batch=L)
             outs.append(x2.view(B, L, D))
         ctx.blk = blk
         ctx.streams = streams
-        ctx.attn = (q, k, v, qhat, khat, q_rstd, k_rstd, o, lse)
+        ctx.attn = (q, k, v, qhat, khat, q_rstd, k_rstd, oa, lse)
         ctx.save_for_backward(temb, cos, sin)
         ctx.dims = (B, Li, Lt, D, H)
         return outs[0], outs[1]
@@ -245,93 +386,77 @@ class FluxDoubleBlockFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, d_hidden, d_enc):
         blk = ctx.blk
+        S = blk.sites
         temb, cos, sin = ctx.saved_tensors
         B, Li, Lt, D, H = ctx.dims
         Ltot = Li + Lt
+        C = H * HD
         dev = temb.device
         bf = torch.bfloat16
-        q, k, v, qhat, khat, q_rstd, k_rstd, o, lse = ctx.attn
-        o3 = o.view(B, Ltot, H * HD)
-        d_o = torch.empty((B * Ltot, H * HD), dtype=bf, device=dev)
-        d_o3 = d_o.view(B, Ltot, H * HD)
-        tail = ((blk.attn.to_out[0], blk.ff), (blk.attn.to_add_out, blk.ff_context))
+        f32 = torch.float32
+        q, k, v, qhat, khat, q_rstd, k_rstd, oa, lse = ctx.attn
+        oa3 = oa.view(B, Ltot, oa.shape[1])
+        d_o = torch.empty((B * Ltot, C), dtype=bf, device=dev)
+        d_o3 = d_o.view(B, Ltot, C)
+        tail = ((S['to_out'], S['ff1'], S['ff2']), (S['to_add_out'], S['ffc1'], S['ffc2']))
         dmods, dx1s = [], []
-        for st, (wo, ff), dxo in zip(ctx.streams, tail, (d_hidden, d_enc)):
+        for st, (swo, s1, s2), dxo in zip(ctx.streams, tail, (d_hidden, d_enc)):
             L, off, m = st.L, st.off, st.mod
             dx2 = dxo.reshape(B * L, D)
             if dx2.dtype != bf:
                 dx2 = dx2.to(bf)
-            dmod = torch.empty((B, 6 * D), dtype=torch.float32, device=dev)
-            w1, w2 = ff.net[0].proj, ff.net[2]
+            dmod = torch.empty((B, 6 * D), dtype=f32, device=dev)
             # ---- MLP branch: x2 = x1 + gate_mlp * (h W2^T + b2) ----
-            dy2, part = ops.gate_bwd(dx2, st.y_mlp, m[:, 5 * D:6 * D], B, L)
-            db2 = torch.empty(D, dtype=torch.float32, device=dev)
+            dy2a = s2.alloc_dy(B * L, dev)
+            _, part = ops.gate_bwd(dx2, st.y_mlp, m[:, 5 * D:6 * D], B, L, dy=dy2a[:, :D])
+            db2 = torch.empty(D, dtype=f32, device=dev) if s2.bias_grad else None
             ops.colreduce_finish(part, per_sample0=dmod[:, 5 * D:6 * D], summed1=db2)
-            du = ops.gemm(dy2, w2.weight, b_mn=True, epilogue=ops.EPI_MUL_GELU_GRAD, aux=st.u)        # [BL, 4D]
-            if w2.weight.requires_grad:
-                def wgrad_w2(w2=w2, dy2=dy2, h=st.h, db2=db2):
-                    g, acc = _grad_buf(w2.weight)
-                    ops.gemm(dy2, h, a_mn=True, b_mn=True, out=g, accumulate=acc)                      # dW2 = dy2^T h
-                    _acc_vec(w2.bias, db2)
-                ops.defer(wgrad_w2)
-            xn2 = st.xn2
-            if w1.weight.requires_grad:
-                db1 = ops.colsum(du)
-
-                def wgrad_w1(w1=w1, du=du, xn2=xn2, db1=db1):
-                    g, acc = _grad_buf(w1.weight)
-                    ops.gemm(du, xn2, a_mn=True, b_mn=True, out=g, accumulate=acc)                     # dW1 = du^T xn2
-                    _acc_vec(w1.bias, db1)
-                ops.defer(wgrad_w1)
-            # (the xn2 storage is recycled for the result unless a deferred weight-gradient still needs xn2)
-            dxn2 = ops.gemm(du, w1.weight, b_mn=True, out=None if ops.deferring() else xn2)
+            s2.backproject(dy2a)
+            dua = s1.alloc_dy(B * L, dev)
+            ops.gemm(dy2a, s2.w_dgrad, b_mn=True, epilogue=ops.EPI_MUL_GELU_GRAD, aux=st.u, out=dua[:, :s1.N])   # [BL, 4D]
+            s2.queue_grads(st.h, dy2a, db2)                                                                   # dW2 = dy2^T h
+            s1.backproject(dua)
+            x2a = s1.rebuild(st.xn2, B * L, dev, lambda out: ops.ln_modulate_fwd(
+                st.x1, m[:, 4 * D:5 * D], m[:, 3 * D:4 * D], B, L, out=out, save_stats=False))
+            s1.queue_grads(x2a, dua, ops.colsum(dua) if s1.bias_grad else None)                             # dW1 = du^T xn2
+            dxn2 = ops.gemm(dua, s1.w_dgrad, b_mn=True, out=s1.dgrad_out(x2a))
             dx1, part = ops.ln_modulate_bwd(dxn2, st.x1, m[:, 4 * D:5 * D], st.mean2, st.rstd2, B, L, dres=dx2)
             ops.colreduce_finish(part, per_sample0=dmod[:, 4 * D:5 * D], per_sample1=dmod[:, 3 * D:4 * D])
             # ---- attention branch: x1 = x + gate_msa * (o W_o^T + b_o) ----
-            dy1, part = ops.gate_bwd(dx1, st.y_attn, m[:, 2 * D:3 * D], B, L, dy=dxn2)
-            dbo = torch.empty(D, dtype=torch.float32, device=dev)
+            dy1a = swo.alloc_dy(B * L, dev, spare=dxn2)
+            _, part = ops.gate_bwd(dx1, st.y_attn, m[:, 2 * D:3 * D], B, L, dy=dy1a[:, :D])
+            dbo = torch.empty(D, dtype=f32, device=dev) if swo.bias_grad else None
             ops.colreduce_finish(part, per_sample0=dmod[:, 2 * D:3 * D], summed1=dbo)
+            swo.backproject(dy1a)
             for b in range(B):
-                rs = slice(b * L, (b + 1) * L)
-                ops.gemm(dy1[rs], wo.weight, b_mn=True, out=d_o3[b, off:off + L])                      # d o (this stream's rows)
-            if wo.weight.requires_grad:
-                def wgrad_wo(wo=wo, dy1=dy1, o3=o3, dbo=dbo, L=L, off=off):
-                    wg, acc = _grad_buf(wo.weight)
-                    for b in range(B):
-                        ops.gemm(dy1[b * L:(b + 1) * L], o3[b, off:off + L], a_mn=True, b_mn=True, out=wg,
-                                 accumulate=acc or b > 0)                                              # dWo = dy1^T o
-                    _acc_vec(wo.bias, dbo)
-                ops.defer(wgrad_wo)
+                ops.gemm(dy1a[b * L:(b + 1) * L], swo.w_dgrad, b_mn=True, out=d_o3[b, off:off + L])       # d o (this stream's rows)
+            swo.queue_grads([oa3[b, off:off + L] for b in range(B)], [dy1a[b * L:(b + 1) * L] for b in range(B)], dbo)
             dmods.append(dmod)
             dx1s.append(dx1)
         if ctx.ragged:
             dq, dk, dv = _ragged_attn_bwd(lse, d_o, q.shape)
         else:
-            dq, dk, dv = ops.attn_bwd(q, k, v, o, d_o, lse)
-        d_temb = torch.zeros_like(temb, dtype=torch.float32)
+            dq, dk, dv = ops.attn_bwd(q, k, v, oa, d_o, lse)
+        d_temb = torch.zeros_like(temb, dtype=f32)
         grads = []
-        spec = ((blk.norm1.linear, blk.qkv, blk.attn.norm_q, blk.attn.norm_k),
-                (blk.norm1_context.linear, blk.add_qkv, blk.attn.norm_added_q, blk.attn.norm_added_k))
-        for st, dmod, dx1, (modlin, fq, nq, nk) in zip(ctx.streams, dmods, dx1s, spec):
+        spec = ((S['mod'], S['qkv'], blk.attn.norm_q, blk.attn.norm_k),
+                (S['mod_c'], S['add_qkv'], blk.attn.norm_added_q, blk.attn.norm_added_k))
+        for st, dmod, dx1, (ml, sq, nq, nk) in zip(ctx.streams, dmods, dx1s, spec):
             L, off, m = st.L, st.off, st.mod
-            dqkv = torch.empty((B * L, 3 * H * HD), dtype=bf, device=dev)
-            dbias = torch.zeros(3 * H * HD, dtype=torch.float32, device=dev)
-            dw = torch.zeros((2, HD), dtype=torch.float32, device=dev)
-            ops.qknorm_rope_bwd(dq, dk, dv, qhat, khat, q_rstd, k_rstd, nq.weight, nk.weight, cos, sin, dqkv, dbias, dw,
+            dqa = sq.alloc_dy(B * L, dev)
+            dbias = torch.zeros(3 * C, dtype=f32, device=dev)
+            dw = torch.zeros((2, HD), dtype=f32, device=dev)
+            ops.qknorm_rope_bwd(dq, dk, dv, qhat, khat, q_rstd, k_rstd, nq.weight, nk.weight, cos, sin, dqa, dbias, dw,
                                 B, H, Ltot, off, L)
-            xn = st.xn
-            if fq.requires_grad():
-                def wgrad_qkv(fq=fq, nq=nq, nk=nk, dqkv=dqkv, xn=xn, dbias=dbias, dw=dw):
-                    wgrad, bgrad, acc = fq.grads()
-                    ops.gemm(dqkv, xn, a_mn=True, b_mn=True, out=wgrad, accumulate=acc)                # dWqkv = dqkv^T xn
-                    _acc_fused_bias(fq, bgrad, acc, dbias)
-                    _acc_vec(nq.weight, dw[0])
-                    _acc_vec(nk.weight, dw[1])
-                ops.defer(wgrad_qkv)
-            dxn = ops.gemm(dqkv, fq.weight, b_mn=True, out=None if ops.deferring() else xn)
+            _defer_acc((nq.weight, dw[0]), (nk.weight, dw[1]))
+            sq.backproject(dqa)
+            xa = sq.rebuild(st.xn, B * L, dev, lambda out: ops.ln_modulate_fwd(
+                st.x, m[:, D:2 * D], m[:, 0:D], B, L, out=out, save_stats=False))
+            sq.queue_grads(xa, dqa, dbias)                                                                    # dWqkv = dqkv^T xn
+            dxn = ops.gemm(dqa, sq.w_dgrad, b_mn=True, out=sq.dgrad_out(xa))
             dx, part = ops.ln_modulate_bwd(dxn, st.x, m[:, D:2 * D], st.mean1, st.rstd1, B, L, dres=dx1)
             ops.colreduce_finish(part, per_sample0=dmod[:, D:2 * D], per_sample1=dmod[:, 0:D])
-            _mod_bwd(dmod, temb, modlin, d_temb)
+            ml.bwd(dmod, temb, st.mod_saved, d_temb)
             grads.append(dx.view(B, L, D))
         ctx.streams = None
         ctx.attn = None
@@ -362,6 +487,14 @@ def _norm_w(dtype, device):
     return m
 
 
+def double_block_sites(mod, mod_c, qkv, add_qkv, attn, ff, ff_context):
+    """the dense `sites` of a double-stream block (FluxDoubleBlockFn); lora.attach_double_block replaces them"""
+    return {'mod': DenseMod(mod), 'mod_c': DenseMod(mod_c), 'qkv': DenseSite(qkv), 'add_qkv': DenseSite(add_qkv),
+            'to_out': DenseSite(attn.to_out[0]), 'to_add_out': DenseSite(attn.to_add_out),
+            'ff1': DenseSite(ff.net[0].proj), 'ff2': DenseSite(ff.net[2]),
+            'ffc1': DenseSite(ff_context.net[0].proj), 'ffc2': DenseSite(ff_context.net[2])}
+
+
 class FluxTransformerBlock(nn.Module):
     """Drop-in for diffusers.models.transformers.transformer_flux.FluxTransformerBlock (same parameter names and
     call signature as used at models/flux.py:502); returns (encoder_hidden_states, hidden_states)."""
@@ -384,13 +517,11 @@ class FluxTransformerBlock(nn.Module):
         self.attn = a
         self.ff = _FF(dim, dim * mlp_ratio, dtype, device)
         self.ff_context = _FF(dim, dim * mlp_ratio, dtype, device)
+        self.sites = double_block_sites(self.norm1.linear, self.norm1_context.linear, self.qkv, self.add_qkv, a, self.ff,
+                                        self.ff_context)
 
     def forward(self, hidden_states, encoder_hidden_states, temb, image_rotary_emb, joint_attention_kwargs=None):
         cos, sin = image_rotary_emb
-        if 'lora' in self.__dict__:          # adapters attached (lora.py): frozen base, K-extended GEMMs
-            from .lora import FluxDoubleBlockLoraFn
-            h, e = FluxDoubleBlockLoraFn.apply(self, hidden_states, encoder_hidden_states, temb, cos, sin, None)
-            return e, h
         h, e = FluxDoubleBlockFn.apply(self, hidden_states, encoder_hidden_states, temb, cos, sin, None)
         return e, h
 
@@ -412,40 +543,44 @@ def _joint(enc, hidden):
 
 
 class FluxSingleBlockFn(torch.autograd.Function):
+    """Flux single-stream block over `blk.sites` (keys: mod, lin1 = [q; k; v; proj_mlp], proj_out)."""
+
     @staticmethod
     def forward(ctx, blk, hidden, enc, temb, cos, sin):
+        S = blk.sites
+        _refresh(S)
         B, Li, D = hidden.shape
         Lt = enc.shape[1]
         L = Li + Lt
         H = blk.heads
         dev = hidden.device
         bf = torch.bfloat16
+        s1, s2 = S['lin1'], S['proj_out']
         x = _joint(enc, hidden).reshape(B * L, D)
-        mod = _mod_fwd(temb, blk.norm.linear)                               # [B, 3D]: shift, scale, gate
-        xn, mean, rstd = ops.ln_modulate_fwd(x, mod[:, D:2 * D], mod[:, 0:D], B, L)
+        mod, mod_saved = S['mod'].fwd(temb)                                 # [B, 3D]: shift, scale, gate
+        xa = s1.alloc_in(B * L, dev)
+        _, mean, rstd = ops.ln_modulate_fwd(x, mod[:, D:2 * D], mod[:, 0:D], B, L, out=xa[:, :D])
+        s1.project(xa)
+        xn = s1.keep(xa)
         shp = (B, H, L, HD)
-        q = torch.empty(shp, dtype=bf, device=dev)
-        k = torch.empty(shp, dtype=bf, device=dev)
-        v = torch.empty(shp, dtype=bf, device=dev)
-        qhat = torch.empty(shp, dtype=bf, device=dev)
-        khat = torch.empty(shp, dtype=bf, device=dev)
+        q, k, v, qhat, khat = (torch.empty(shp, dtype=bf, device=dev) for _ in range(5))
         q_rstd = torch.empty((B, H, L), dtype=torch.float32, device=dev)
         k_rstd = torch.empty((B, H, L), dtype=torch.float32, device=dev)
         inner = blk.mlp_dim
-        cat = torch.empty((B * L, D + inner), dtype=bf, device=dev)      # [attn | gelu(mlp)]: the operand of proj_out
+        cata = s2.alloc_in(B * L, dev)              # [attn | gelu(mlp) (| adapter columns)]: the operand of proj_out
         u = torch.empty((B * L, inner), dtype=bf, device=dev)
-        f1 = blk.lin1
         e = ops.make_qkv_epilogue(q, k, v, blk.attn.norm_q.weight, blk.attn.norm_k.weight, cos, sin, H, L, 0, qhat, khat,
                                   q_rstd, k_rstd)
-        ops.gemm(xn, f1.weight, bias=f1.bias, epilogue=ops.EPI_QKV_ROPE, out=cat[:, D:], out2=u, rows_per_batch=L, qkv=e)
-        _, lse = ops.attn_fwd(q, k, v, out=cat)
+        ops.gemm(xa, s1.w_fwd, bias=s1.bias, epilogue=ops.EPI_QKV_ROPE, out=cata[:, D:D + inner], out2=u, rows_per_batch=L,
+                 qkv=e)
+        _, lse = ops.attn_fwd(q, k, v, out=cata)
+        s2.project(cata)
         y = torch.empty((B * L, D), dtype=bf, device=dev)
-        po = blk.proj_out
-        xo = ops.gemm(cat, po.weight, bias=po.bias, epilogue=ops.EPI_GATE_RES, aux=x, gate=mod[:, 2 * D:3 * D], out2=y,
+        xo = ops.gemm(cata, s2.w_fwd, bias=s2.bias, epilogue=ops.EPI_GATE_RES, aux=x, gate=mod[:, 2 * D:3 * D], out2=y,
                       rows_per_batch=L)
         xo3 = xo.view(B, L, D)
         ctx.blk = blk
-        ctx.saved = (x, mod, mean, rstd, q, k, v, qhat, khat, q_rstd, k_rstd, cat, u, lse, y, xn)
+        ctx.saved = (x, mod, mod_saved, mean, rstd, xn, q, k, v, qhat, khat, q_rstd, k_rstd, cata, u, lse, y)
         ctx.save_for_backward(temb, cos, sin)
         ctx.dims = (B, Li, Lt, D, H)
         return xo3[:, Lt:], xo3[:, :Lt]
@@ -453,52 +588,49 @@ class FluxSingleBlockFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, d_hidden, d_enc):
         blk = ctx.blk
+        S = blk.sites
         temb, cos, sin = ctx.saved_tensors
         B, Li, Lt, D, H = ctx.dims
         L = Li + Lt
+        C = H * HD
         dev = temb.device
         bf = torch.bfloat16
-        x, mod, mean, rstd, q, k, v, qhat, khat, q_rstd, k_rstd, cat, u, lse, y, xn = ctx.saved
+        f32 = torch.float32
+        x, mod, mod_saved, mean, rstd, xn, q, k, v, qhat, khat, q_rstd, k_rstd, cata, u, lse, y = ctx.saved
+        s1, s2 = S['lin1'], S['proj_out']
         inner = blk.mlp_dim
         dxo = _joint(d_enc, d_hidden).reshape(B * L, D)
         if dxo.dtype != bf:
             dxo = dxo.to(bf)
-        dmod = torch.empty((B, 3 * D), dtype=torch.float32, device=dev)
-        po, f1 = blk.proj_out, blk.lin1
-        dy, part = ops.gate_bwd(dxo, y, mod[:, 2 * D:3 * D], B, L)
-        dbo = torch.empty(D, dtype=torch.float32, device=dev)
+        dmod = torch.empty((B, 3 * D), dtype=f32, device=dev)
+        dya = s2.alloc_dy(B * L, dev)
+        _, part = ops.gate_bwd(dxo, y, mod[:, 2 * D:3 * D], B, L, dy=dya[:, :D])
+        dbo = torch.empty(D, dtype=f32, device=dev) if s2.bias_grad else None
         ops.colreduce_finish(part, per_sample0=dmod[:, 2 * D:3 * D], summed1=dbo)
-        n1 = 3 * H * HD + inner
-        dlin1 = torch.empty((B * L, n1), dtype=bf, device=dev)           # [dq | dk | dv | d mlp_pre]
+        s2.backproject(dya)
+        dl1a = s1.alloc_dy(B * L, dev)                                   # [dq | dk | dv | d mlp_pre (| adapter columns)]
         d_o = torch.empty((B * L, D), dtype=bf, device=dev)
-        ops.gemm(dy, po.weight[:, :D], b_mn=True, out=d_o)                                              # d attn
-        ops.gemm(dy, po.weight[:, D:], b_mn=True, epilogue=ops.EPI_MUL_GELU_GRAD, aux=u, out=dlin1[:, 3 * H * HD:])
-        if po.weight.requires_grad:
-            def wgrad_po(po=po, dy=dy, cat=cat, dbo=dbo):
-                g, acc = _grad_buf(po.weight)
-                ops.gemm(dy, cat, a_mn=True, b_mn=True, out=g, accumulate=acc)
-                _acc_vec(po.bias, dbo)
-            ops.defer(wgrad_po)
-        dq, dk, dv = ops.attn_bwd(q, k, v, cat, d_o, lse)
-        dbias = torch.zeros(n1, dtype=torch.float32, device=dev)
-        dw = torch.zeros((2, HD), dtype=torch.float32, device=dev)
+        wd = s2.w_dgrad                                                  # [D (+ R), D + inner]
+        ops.gemm(dya, wd[:, :D], b_mn=True, out=d_o)                                                     # d attn
+        ops.gemm(dya, wd[:, D:], b_mn=True, epilogue=ops.EPI_MUL_GELU_GRAD, aux=u, out=dl1a[:, 3 * C:3 * C + inner])
+        s2.queue_grads(cata, dya, dbo)
+        dq, dk, dv = ops.attn_bwd(q, k, v, cata, d_o, lse)
+        dbias = torch.zeros(3 * C + inner, dtype=f32, device=dev)
+        dw = torch.zeros((2, HD), dtype=f32, device=dev)
         ops.qknorm_rope_bwd(dq, dk, dv, qhat, khat, q_rstd, k_rstd, blk.attn.norm_q.weight, blk.attn.norm_k.weight, cos,
-                            sin, dlin1, dbias[:3 * H * HD], dw, B, H, L, 0, L)
-        if f1.requires_grad():
-            ops.colsum(dlin1[:, 3 * H * HD:], out=dbias[3 * H * HD:])
-
-            def wgrad_lin1(f1=f1, blk=blk, dlin1=dlin1, xn=xn, dbias=dbias, dw=dw):
-                wgrad, bgrad, acc = f1.grads()
-                ops.gemm(dlin1, xn, a_mn=True, b_mn=True, out=wgrad, accumulate=acc)
-                _acc_fused_bias(f1, bgrad, acc, dbias)
-                _acc_vec(blk.attn.norm_q.weight, dw[0])
-                _acc_vec(blk.attn.norm_k.weight, dw[1])
-            ops.defer(wgrad_lin1)
-        dxn = ops.gemm(dlin1, f1.weight, b_mn=True, out=None if ops.deferring() else xn)
+                            sin, dl1a, dbias[:3 * C], dw, B, H, L, 0, L)
+        _defer_acc((blk.attn.norm_q.weight, dw[0]), (blk.attn.norm_k.weight, dw[1]))
+        if s1.bias_grad:
+            ops.colsum(dl1a[:, 3 * C:3 * C + inner], out=dbias[3 * C:])
+        s1.backproject(dl1a)
+        xa = s1.rebuild(xn, B * L, dev, lambda out: ops.ln_modulate_fwd(
+            x, mod[:, D:2 * D], mod[:, 0:D], B, L, out=out, save_stats=False))
+        s1.queue_grads(xa, dl1a, dbias)
+        dxn = ops.gemm(dl1a, s1.w_dgrad, b_mn=True, out=s1.dgrad_out(xa))
         dx, part = ops.ln_modulate_bwd(dxn, x, mod[:, D:2 * D], mean, rstd, B, L, dres=dxo)
         ops.colreduce_finish(part, per_sample0=dmod[:, D:2 * D], per_sample1=dmod[:, 0:D])
-        d_temb = torch.zeros((B, D), dtype=torch.float32, device=dev)
-        _mod_bwd(dmod, temb, blk.norm.linear, d_temb)
+        d_temb = torch.zeros((B, D), dtype=f32, device=dev)
+        S['mod'].bwd(dmod, temb, mod_saved, d_temb)
         dx3 = dx.view(B, L, D)
         ctx.saved = None
         return None, dx3[:, Lt:], dx3[:, :Lt], d_temb.to(temb.dtype), None, None
@@ -520,12 +652,9 @@ class FluxSingleTransformerBlock(nn.Module):
         self.attn = a
         self.proj_mlp = self.lin1.lin(3)
         self.proj_out = _plain(dim, dim + self.mlp_dim, dtype, device)
+        self.sites = {'mod': DenseMod(self.norm.linear), 'lin1': DenseSite(self.lin1), 'proj_out': DenseSite(self.proj_out)}
 
     def forward(self, hidden_states, encoder_hidden_states, temb, image_rotary_emb, joint_attention_kwargs=None):
         cos, sin = image_rotary_emb
-        if 'lora' in self.__dict__:
-            from .lora import FluxSingleBlockLoraFn
-            h, e = FluxSingleBlockLoraFn.apply(self, hidden_states, encoder_hidden_states, temb, cos, sin)
-            return e, h
         h, e = FluxSingleBlockFn.apply(self, hidden_states, encoder_hidden_states, temb, cos, sin)
         return e, h

@@ -33,7 +33,7 @@ from torch import nn
 
 from . import ops
 from .flux import AdaLNContinuousFn, MseLossFn, _MLPEmbedder, get_lin_function, linear, make_contiguous, time_shift
-from .flux_blocks import HD, FluxDoubleBlockFn, FusedParam, _AdaNorm, _Attn, _FF, _norm_w, _plain
+from .flux_blocks import HD, FluxDoubleBlockFn, FusedParam, _AdaNorm, _Attn, _FF, _norm_w, _plain, double_block_sites
 from .plugin import PluginSurface
 
 QWEN_IMAGE_CONFIG = {   # reference: configs/qwen_image/transformer/config.json
@@ -71,21 +71,18 @@ class QwenImageTransformerBlock(nn.Module):
         self.attn = a
         self.img_mlp = _FF(dim, dim * mlp_ratio, dtype, device)
         self.txt_mlp = _FF(dim, dim * mlp_ratio, dtype, device)
-        # the names FluxDoubleBlockFn reads (plain attributes: no second registration of the same parameters)
+        # the Flux names lora.attach_double_block reads (plain attributes: no second registration of the same parameters)
         d = self.__dict__
         d['qkv'], d['add_qkv'] = qkv, add_qkv
         d['norm1'] = _Alias(linear=self.img_mod[1])
         d['norm1_context'] = _Alias(linear=self.txt_mod[1])
         d['ff'], d['ff_context'] = self.img_mlp, self.txt_mlp
+        self.sites = double_block_sites(self.img_mod[1], self.txt_mod[1], qkv, add_qkv, a, self.img_mlp, self.txt_mlp)
 
     def forward(self, hidden_states, encoder_hidden_states, temb, image_rotary_emb, encoder_hidden_states_mask=None,
                 joint_attention_kwargs=None, txt_lens=None):
         """txt_lens: None, or the real prompt length of every sample when the micro-batch is padded (key mask)"""
         cos, sin = image_rotary_emb            # joint [text; image] tables, fp32 [L, 128]
-        if 'lora' in self.__dict__:
-            from .lora import FluxDoubleBlockLoraFn
-            h, e = FluxDoubleBlockLoraFn.apply(self, hidden_states, encoder_hidden_states, temb, cos, sin, txt_lens)
-            return e, h
         h, e = FluxDoubleBlockFn.apply(self, hidden_states, encoder_hidden_states, temb, cos, sin, txt_lens)
         return e, h
 

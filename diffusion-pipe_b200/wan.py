@@ -11,6 +11,9 @@ A WanAttentionBlock (models/wan/model.py:242-318) is ONE torch.autograd.Function
 GELU / gated-residual epilogues, the fused attention kernels (self-attention over the video tokens with RoPE,
 cross-attention over the 512 text slots), the LayerNorm+modulation kernels in their "bf16 after every op" mode (the
 block's operands are all bf16 tensors in the reference) and the full-width RMSNorm+RoPE kernels of csrc/wan_norm.cu.
+Like the Flux blocks it reads its GEMMs through `blk.sites` (flux_blocks.DenseSite, or lora.LoraSite once adapters are
+attached), so dense and LoRA training run the same function.  Its three LayerNorm+modulation outputs are recomputed in
+backward (DESIGN.md §3).
 Scope: model_type 't2v' (Wan2.1 / Wan2.2 T2V) and 'i2v_v2' (Wan2.2 I2V: first-frame mask + conditioning latents as extra
 input channels), both cross_attn_type 'default', with cached text embeddings; Wan2.1 i2v / flf2v (CLIP image context)
 and ti2v (per-token timesteps) raise NotImplementedError.
@@ -28,7 +31,7 @@ from torch import nn
 
 from . import ops
 from .flux import linear, make_contiguous
-from .flux_blocks import HD, FusedParam, _acc_vec, _grad_buf, _mod_bwd, _mod_fwd, _plain
+from .flux_blocks import HD, DenseSite, FusedParam, _acc_vec, _defer_acc, _grad_buf, _mod_bwd, _mod_fwd, _plain, _refresh
 from .plugin import PluginSurface
 
 WAN_T2V_14B_CONFIG = {   # reference: models/wan/configs.py:60-75 (t2v_14B)
@@ -126,56 +129,83 @@ class LnModFn(torch.autograd.Function):
 # the block
 # =====================================================================================================================
 class WanBlockFn(torch.autograd.Function):
+    """Wan attention block over `blk.sites` (keys: sa_qkv, sa_o, ca_q, ca_kv, ca_o, ffn1, ffn2)."""
+
     @staticmethod
     def forward(ctx, blk, x, e0, context, cos, sin):
+        S = blk.sites
+        _refresh(S)
         B, L, D = x.shape
         Lc = context.shape[1]
         H = blk.num_heads
         dev = x.device
         bf = torch.bfloat16
+        LN_STEPS, LN_MULT = ops.LN_ROUND_STEPS, ops.LN_MULT_DIRECT
         x2 = x.reshape(B * L, D)
         c2 = context.reshape(B * Lc, D)
         if c2.dtype != bf:
             c2 = c2.to(bf)
         mod = (blk.modulation.unsqueeze(0) + e0).reshape(B, 6, D)      # bf16 + bf16 -> bf16, as the reference (:298)
         sa, ca = blk.self_attn, blk.cross_attn
+        s_qkv, s_o, s_cq, s_ckv, s_co, s_f1, s_f2 = (S[k] for k in ('sa_qkv', 'sa_o', 'ca_q', 'ca_kv', 'ca_o', 'ffn1', 'ffn2'))
+        # the LayerNorm outputs that feed the sites are recomputed in backward (keep(recompute=True)); a dense site's
+        # buffer is recycled as the output of the next residual GEMM (x1, x3)
         # ---- self-attention ----
-        xn1, mean1, rstd1 = ops.ln_modulate_fwd(x2, mod[:, 1], mod[:, 0], B, L, eps=blk.eps, flags=ops.LN_ROUND_STEPS)
-        qkv = ops.gemm(xn1, sa.qkv.weight, bias=sa.qkv.bias)
+        xa = s_qkv.alloc_in(B * L, dev)
+        _, mean1, rstd1 = ops.ln_modulate_fwd(x2, mod[:, 1], mod[:, 0], B, L, eps=blk.eps, out=xa[:, :D], flags=LN_STEPS)
+        s_qkv.project(xa)
+        kept1 = s_qkv.keep(xa, recompute=True)
+        qkv = ops.gemm(xa, s_qkv.w_fwd, bias=s_qkv.bias)
         (q, xhq, rq), (k, xhk, rk), (v, _, _) = ops.wan_norm_rope_fwd(
             [{'src': qkv[:, 0:D], 'weight': sa.norm_q.weight, 'rope': True},
              {'src': qkv[:, D:2 * D], 'weight': sa.norm_k.weight, 'rope': True},
              {'src': qkv[:, 2 * D:3 * D]}], B, L, H, cos, sin, eps=blk.eps)
-        del qkv
-        o, lse = ops.attn_fwd(q, k, v)
+        spare = s_qkv.spare(xa)
+        del qkv, xa
+        oa = s_o.alloc_in(B * L, dev)
+        _, lse = ops.attn_fwd(q, k, v, out=oa)
+        s_o.project(oa)
         y_attn = torch.empty((B * L, D), dtype=bf, device=dev)
-        x1 = ops.gemm(o, sa.o.weight, bias=sa.o.bias, epilogue=ops.EPI_GATE_RES, aux=x2, gate=mod[:, 2], out2=y_attn,
-                      rows_per_batch=L, out=xn1)
+        x1 = ops.gemm(oa, s_o.w_fwd, bias=s_o.bias, epilogue=ops.EPI_GATE_RES, aux=x2, gate=mod[:, 2], out2=y_attn,
+                      rows_per_batch=L, out=spare)
         # ---- cross-attention (text context; all text_len slots attended: context_lens=None at models/wan/wan.py:526) ----
         n3w = blk.norm3.weight.view(1, D).expand(B, D)
         n3b = blk.norm3.bias.view(1, D).expand(B, D)
-        xn3, mean3, rstd3 = ops.ln_modulate_fwd(x1, n3w, n3b, B, L, eps=blk.eps, flags=ops.LN_MULT_DIRECT)
-        qc_lin = ops.gemm(xn3, ca.q.weight, bias=ca.q.bias)
+        x3a = s_cq.alloc_in(B * L, dev)
+        _, mean3, rstd3 = ops.ln_modulate_fwd(x1, n3w, n3b, B, L, eps=blk.eps, out=x3a[:, :D], flags=LN_MULT)
+        s_cq.project(x3a)
+        kept3 = s_cq.keep(x3a, recompute=True)
+        qc_lin = ops.gemm(x3a, s_cq.w_fwd, bias=s_cq.bias)
         ((qc, xhqc, rqc),) = ops.wan_norm_rope_fwd([{'src': qc_lin, 'weight': ca.norm_q.weight}], B, L, H, eps=blk.eps)
-        del qc_lin, xn3
-        kv_lin = ops.gemm(c2, ca.kv.weight, bias=ca.kv.bias)
+        del qc_lin, x3a
+        ca_in = s_ckv.input_operand(c2)
+        kv_lin = ops.gemm(ca_in, s_ckv.w_fwd, bias=s_ckv.bias)
         (kc, xhkc, rkc), (vc, _, _) = ops.wan_norm_rope_fwd(
             [{'src': kv_lin[:, 0:D], 'weight': ca.norm_k.weight}, {'src': kv_lin[:, D:2 * D]}], B, Lc, H, eps=blk.eps)
         del kv_lin
-        oc, lse_c = ops.attn_fwd(qc, kc, vc)
-        x2_ = ops.gemm(oc, ca.o.weight, bias=ca.o.bias, epilogue=ops.EPI_GATE_RES, aux=x1, gate=blk._ones(B, D, dev),
+        oca = s_co.alloc_in(B * L, dev)
+        _, lse_c = ops.attn_fwd(qc, kc, vc, out=oca)
+        s_co.project(oca)
+        x2_ = ops.gemm(oca, s_co.w_fwd, bias=s_co.bias, epilogue=ops.EPI_GATE_RES, aux=x1, gate=blk._ones(B, D, dev),
                        rows_per_batch=L)
         # ---- feed-forward ----
-        xn2, mean2, rstd2 = ops.ln_modulate_fwd(x2_, mod[:, 4], mod[:, 3], B, L, eps=blk.eps, flags=ops.LN_ROUND_STEPS)
-        w1, w2 = blk.ffn[0], blk.ffn[2]
-        u = torch.empty((B * L, w1.weight.shape[0]), dtype=bf, device=dev)
-        h = ops.gemm(xn2, w1.weight, bias=w1.bias, epilogue=ops.EPI_BIAS_GELU, out2=u)
+        x2a = s_f1.alloc_in(B * L, dev)
+        _, mean2, rstd2 = ops.ln_modulate_fwd(x2_, mod[:, 4], mod[:, 3], B, L, eps=blk.eps, out=x2a[:, :D], flags=LN_STEPS)
+        s_f1.project(x2a)
+        kept2 = s_f1.keep(x2a, recompute=True)
+        F = s_f1.N
+        u = torch.empty((B * L, F), dtype=bf, device=dev)
+        ha = s_f2.alloc_in(B * L, dev)
+        ops.gemm(x2a, s_f1.w_fwd, bias=s_f1.bias, epilogue=ops.EPI_BIAS_GELU, out=ha[:, :F], out2=u)
+        spare = s_f1.spare(x2a)
+        del x2a
+        s_f2.project(ha)
         y_mlp = torch.empty((B * L, D), dtype=bf, device=dev)
-        x3 = ops.gemm(h, w2.weight, bias=w2.bias, epilogue=ops.EPI_GATE_RES, aux=x2_, gate=mod[:, 5], out2=y_mlp,
-                      rows_per_batch=L, out=xn2)
+        x3 = ops.gemm(ha, s_f2.w_fwd, bias=s_f2.bias, epilogue=ops.EPI_GATE_RES, aux=x2_, gate=mod[:, 5], out2=y_mlp,
+                      rows_per_batch=L, out=spare)
         ctx.blk = blk
-        ctx.saved = (x2, c2, mod, mean1, rstd1, q, k, v, xhq, rq, xhk, rk, o, lse, y_attn, x1, mean3, rstd3, qc, xhqc, rqc,
-                     kc, xhkc, rkc, vc, oc, lse_c, x2_, mean2, rstd2, u, h, y_mlp)
+        ctx.saved = (x2, c2, mod, mean1, rstd1, kept1, q, k, v, xhq, rq, xhk, rk, oa, lse, y_attn, x1, mean3, rstd3, kept3,
+                     qc, xhqc, rqc, ca_in, kc, xhkc, rkc, vc, oca, lse_c, x2_, mean2, rstd2, kept2, u, ha, y_mlp)
         ctx.save_for_backward(cos, sin)
         ctx.dims = (B, L, Lc, D, H)
         ctx.in_dtypes = (x.dtype, e0.dtype, context.dtype)
@@ -184,124 +214,99 @@ class WanBlockFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dx3):
         blk = ctx.blk
+        S = blk.sites
         cos, sin = ctx.saved_tensors
         B, L, Lc, D, H = ctx.dims
-        (x2, c2, mod, mean1, rstd1, q, k, v, xhq, rq, xhk, rk, o, lse, y_attn, x1, mean3, rstd3, qc, xhqc, rqc,
-         kc, xhkc, rkc, vc, oc, lse_c, x2_, mean2, rstd2, u, h, y_mlp) = ctx.saved
+        (x2, c2, mod, mean1, rstd1, kept1, q, k, v, xhq, rq, xhk, rk, oa, lse, y_attn, x1, mean3, rstd3, kept3,
+         qc, xhqc, rqc, ca_in, kc, xhkc, rkc, vc, oca, lse_c, x2_, mean2, rstd2, kept2, u, ha, y_mlp) = ctx.saved
         ctx.saved = None
         dev = x2.device
         bf = torch.bfloat16
+        f32 = torch.float32
+        LN_STEPS, LN_MULT = ops.LN_ROUND_STEPS, ops.LN_MULT_DIRECT
         sa, ca = blk.self_attn, blk.cross_attn
-        w1, w2 = blk.ffn[0], blk.ffn[2]
-        dmod = torch.zeros((B, 6, D), dtype=torch.float32, device=dev)
+        s_qkv, s_o, s_cq, s_ckv, s_co, s_f1, s_f2 = (S[k] for k in ('sa_qkv', 'sa_o', 'ca_q', 'ca_kv', 'ca_o', 'ffn1', 'ffn2'))
+        F = s_f1.N
+        dmod = torch.zeros((B, 6, D), dtype=f32, device=dev)
         d3 = dx3.reshape(B * L, D)
         if d3.dtype != bf:
             d3 = d3.to(bf)
         d3 = d3.contiguous()
         # ---- feed-forward: x3 = x2 + gate5 * (h W2^T + b2) ----
-        dy2, part = ops.gate_bwd(d3, y_mlp, mod[:, 5], B, L)
-        db2 = torch.empty(D, dtype=torch.float32, device=dev)
+        dy2a = s_f2.alloc_dy(B * L, dev)
+        _, part = ops.gate_bwd(d3, y_mlp, mod[:, 5], B, L, dy=dy2a[:, :D])
+        db2 = torch.empty(D, dtype=f32, device=dev) if s_f2.bias_grad else None
         ops.colreduce_finish(part, per_sample0=dmod[:, 5], summed1=db2)
-        du = ops.gemm(dy2, w2.weight, b_mn=True, epilogue=ops.EPI_MUL_GELU_GRAD, aux=u)
-        if w2.weight.requires_grad:
-            def wgrad_w2(w2=w2, dy2=dy2, h=h, db2=db2):
-                g, acc = _grad_buf(w2.weight)
-                ops.gemm(dy2, h, a_mn=True, b_mn=True, out=g, accumulate=acc)
-                _acc_vec(w2.bias, db2)
-            ops.defer(wgrad_w2)
-        xn2, _, _ = ops.ln_modulate_fwd(x2_, mod[:, 4], mod[:, 3], B, L, eps=blk.eps, save_stats=False, flags=ops.LN_ROUND_STEPS)
-        if w1.weight.requires_grad:
-            db1 = ops.colsum(du)
-
-            def wgrad_w1(w1=w1, du=du, xn2=xn2, db1=db1):
-                g, acc = _grad_buf(w1.weight)
-                ops.gemm(du, xn2, a_mn=True, b_mn=True, out=g, accumulate=acc)
-                _acc_vec(w1.bias, db1)
-            ops.defer(wgrad_w1)
-        dxn2 = ops.gemm(du, w1.weight, b_mn=True, out=None if ops.deferring() else xn2)
-        dx2, part = ops.ln_modulate_bwd(dxn2, x2_, mod[:, 4], mean2, rstd2, B, L, dres=d3, flags=ops.LN_ROUND_STEPS)
+        s_f2.backproject(dy2a)
+        dua = s_f1.alloc_dy(B * L, dev)
+        ops.gemm(dy2a, s_f2.w_dgrad, b_mn=True, epilogue=ops.EPI_MUL_GELU_GRAD, aux=u, out=dua[:, :F])
+        s_f2.queue_grads(ha, dy2a, db2)
+        s_f1.backproject(dua)
+        x2a = s_f1.rebuild(kept2, B * L, dev, lambda out: ops.ln_modulate_fwd(
+            x2_, mod[:, 4], mod[:, 3], B, L, eps=blk.eps, out=out, save_stats=False, flags=LN_STEPS))
+        s_f1.queue_grads(x2a, dua, ops.colsum(dua) if s_f1.bias_grad else None)
+        dxn2 = ops.gemm(dua, s_f1.w_dgrad, b_mn=True, out=s_f1.dgrad_out(x2a))
+        # d x2 lands directly in the dy operand of the cross-attention output projection (x2 = x1 + o_c W^T: no gate)
+        dca = s_co.alloc_dy(B * L, dev)
+        _, part = ops.ln_modulate_bwd(dxn2, x2_, mod[:, 4], mean2, rstd2, B, L, dres=d3, dx=dca[:, :D], flags=LN_STEPS)
         ops.colreduce_finish(part, per_sample0=dmod[:, 4], per_sample1=dmod[:, 3])
+        dx2 = dca[:, :D]
         # ---- cross-attention: x2 = x1 + (oc Wo^T + bo) ----
-        d_oc = ops.gemm(dx2, ca.o.weight, b_mn=True)
-        if ca.o.weight.requires_grad:
-            dbo_c = ops.colsum(dx2)
-
-            def wgrad_co(lin=ca.o, dx2=dx2, oc=oc, dbo_c=dbo_c):
-                g, acc = _grad_buf(lin.weight)
-                ops.gemm(dx2, oc, a_mn=True, b_mn=True, out=g, accumulate=acc)
-                _acc_vec(lin.bias, dbo_c)
-            ops.defer(wgrad_co)
-        dqc, dkc, dvc = ops.attn_bwd(qc, kc, vc, oc, d_oc, lse_c)
-        dqc_lin = torch.empty((B * L, D), dtype=bf, device=dev)
-        (dw_nqc,) = ops.wan_norm_rope_bwd([{'dy': dqc, 'dx': dqc_lin, 'weight': ca.norm_q.weight, 'xhat': xhqc, 'rstd': rqc}], B, L, H)
-        dkv_lin = torch.empty((B * Lc, 2 * D), dtype=bf, device=dev)
-        dw_nkc, _ = ops.wan_norm_rope_bwd([{'dy': dkc, 'dx': dkv_lin[:, 0:D], 'weight': ca.norm_k.weight, 'xhat': xhkc, 'rstd': rkc},
-                                           {'dy': dvc, 'dx': dkv_lin[:, D:2 * D]}], B, Lc, H)
+        s_co.backproject(dca)
+        d_oc = ops.gemm(dca, s_co.w_dgrad, b_mn=True)
+        s_co.queue_grads(oca, dca, ops.colsum(dca) if s_co.bias_grad else None)
+        dqc, dkc, dvc = ops.attn_bwd(qc, kc, vc, oca, d_oc, lse_c)
+        dqca = s_cq.alloc_dy(B * L, dev)
+        (dw_nqc,) = ops.wan_norm_rope_bwd([{'dy': dqc, 'dx': dqca[:, :D], 'weight': ca.norm_q.weight, 'xhat': xhqc, 'rstd': rqc}],
+                                          B, L, H)
+        s_cq.backproject(dqca)
+        dkva = s_ckv.alloc_dy(B * Lc, dev)
+        dw_nkc, _ = ops.wan_norm_rope_bwd([{'dy': dkc, 'dx': dkva[:, 0:D], 'weight': ca.norm_k.weight, 'xhat': xhkc, 'rstd': rkc},
+                                           {'dy': dvc, 'dx': dkva[:, D:2 * D]}], B, Lc, H)
+        s_ckv.backproject(dkva)
         n3w = blk.norm3.weight.view(1, D).expand(B, D)
         n3b = blk.norm3.bias.view(1, D).expand(B, D)
-        xn3, _, _ = ops.ln_modulate_fwd(x1, n3w, n3b, B, L, eps=blk.eps, save_stats=False, flags=ops.LN_MULT_DIRECT)
-        if ca.q.weight.requires_grad:
-            dbq_c = ops.colsum(dqc_lin)
-            dbkv_c = ops.colsum(dkv_lin)
-            if ops.deferring():
-                # `context` arrives from the previous stage as a view of a stage-link mailbox slot, which is handed back
-                # to the sender once this input-gradient pass has been enqueued: a weight-gradient closure that runs
-                # later must own its copy (5 MB).  Nothing else a closure captures is a boundary tensor.
-                c2 = c2.clone()
-
-            def wgrad_cq(ca=ca, dqc_lin=dqc_lin, xn3=xn3, dbq_c=dbq_c, dkv_lin=dkv_lin, c2=c2, dbkv_c=dbkv_c, dw_nqc=dw_nqc, dw_nkc=dw_nkc):
-                g, acc = _grad_buf(ca.q.weight)
-                ops.gemm(dqc_lin, xn3, a_mn=True, b_mn=True, out=g, accumulate=acc)
-                _acc_vec(ca.q.bias, dbq_c)
-                wg, bg, acc = ca.kv.grads()
-                ops.gemm(dkv_lin, c2, a_mn=True, b_mn=True, out=wg, accumulate=acc)
-                if acc:
-                    bg.add_(dbkv_c)
-                else:
-                    bg.copy_(dbkv_c)
-                _acc_vec(ca.norm_q.weight, dw_nqc)
-                _acc_vec(ca.norm_k.weight, dw_nkc)
-            ops.defer(wgrad_cq)
-        d_ctx = ops.gemm(dkv_lin, ca.kv.weight, b_mn=True)
-        dxn3 = ops.gemm(dqc_lin, ca.q.weight, b_mn=True, out=None if ops.deferring() else xn3)
-        dx1, part = ops.ln_modulate_bwd(dxn3, x1, n3w, mean3, rstd3, B, L, dres=dx2, flags=ops.LN_MULT_DIRECT)
-        dn3 = torch.empty((2, D), dtype=torch.float32, device=dev)
-        ops.colreduce_finish(part, summed0=dn3[0], summed1=dn3[1])
-        _acc_vec(blk.norm3.weight, dn3[0])
-        _acc_vec(blk.norm3.bias, dn3[1])
+        x3a = s_cq.rebuild(kept3, B * L, dev, lambda out: ops.ln_modulate_fwd(
+            x1, n3w, n3b, B, L, eps=blk.eps, out=out, save_stats=False, flags=LN_MULT))
+        dbq_c = ops.colsum(dqca) if s_cq.bias_grad else None
+        dbkv_c = ops.colsum(dkva) if s_ckv.bias_grad else None
+        if ca_in is c2 and ops.deferring():
+            # `context` arrives from the previous stage as a view of a stage-link mailbox slot, which is handed back
+            # to the sender once this input-gradient pass has been enqueued: a weight-gradient closure that runs
+            # later must own its copy (5 MB).  Nothing else a closure captures is a boundary tensor.
+            ca_in = ca_in.clone()
+        s_cq.queue_grads(x3a, dqca, dbq_c)
+        s_ckv.queue_grads(ca_in, dkva, dbkv_c)
+        _defer_acc((ca.norm_q.weight, dw_nqc), (ca.norm_k.weight, dw_nkc))
+        d_ctx = ops.gemm(dkva, s_ckv.w_dgrad, b_mn=True)
+        dxn3 = ops.gemm(dqca, s_cq.w_dgrad, b_mn=True, out=s_cq.dgrad_out(x3a))
+        dx1, part = ops.ln_modulate_bwd(dxn3, x1, n3w, mean3, rstd3, B, L, dres=dx2, flags=LN_MULT)
+        if blk.norm3.weight.requires_grad:
+            dn3 = torch.empty((2, D), dtype=f32, device=dev)
+            ops.colreduce_finish(part, summed0=dn3[0], summed1=dn3[1])
+            _acc_vec(blk.norm3.weight, dn3[0])
+            _acc_vec(blk.norm3.bias, dn3[1])
         # ---- self-attention: x1 = x + gate2 * (o Wo^T + bo) ----
-        dy1, part = ops.gate_bwd(dx1, y_attn, mod[:, 2], B, L, dy=dxn3)
-        dbo = torch.empty(D, dtype=torch.float32, device=dev)
+        dy1a = s_o.alloc_dy(B * L, dev, spare=dxn3)
+        _, part = ops.gate_bwd(dx1, y_attn, mod[:, 2], B, L, dy=dy1a[:, :D])
+        dbo = torch.empty(D, dtype=f32, device=dev) if s_o.bias_grad else None
         ops.colreduce_finish(part, per_sample0=dmod[:, 2], summed1=dbo)
-        d_o = ops.gemm(dy1, sa.o.weight, b_mn=True)
-        if sa.o.weight.requires_grad:
-            def wgrad_so(lin=sa.o, dy1=dy1, o=o, dbo=dbo):
-                g, acc = _grad_buf(lin.weight)
-                ops.gemm(dy1, o, a_mn=True, b_mn=True, out=g, accumulate=acc)
-                _acc_vec(lin.bias, dbo)
-            ops.defer(wgrad_so)
-        dq, dk, dv = ops.attn_bwd(q, k, v, o, d_o, lse)
-        dqkv = torch.empty((B * L, 3 * D), dtype=bf, device=dev)
+        s_o.backproject(dy1a)
+        d_o = ops.gemm(dy1a, s_o.w_dgrad, b_mn=True)
+        s_o.queue_grads(oa, dy1a, dbo)
+        dq, dk, dv = ops.attn_bwd(q, k, v, oa, d_o, lse)
+        dqkva = s_qkv.alloc_dy(B * L, dev)
         dw_nq, dw_nk, _ = ops.wan_norm_rope_bwd(
-            [{'dy': dq, 'dx': dqkv[:, 0:D], 'weight': sa.norm_q.weight, 'xhat': xhq, 'rstd': rq, 'rope': True},
-             {'dy': dk, 'dx': dqkv[:, D:2 * D], 'weight': sa.norm_k.weight, 'xhat': xhk, 'rstd': rk, 'rope': True},
-             {'dy': dv, 'dx': dqkv[:, 2 * D:3 * D]}], B, L, H, cos, sin)
-        xn1, _, _ = ops.ln_modulate_fwd(x2, mod[:, 1], mod[:, 0], B, L, eps=blk.eps, save_stats=False, flags=ops.LN_ROUND_STEPS)
-        if sa.qkv.requires_grad():
-            dbqkv = ops.colsum(dqkv)
-
-            def wgrad_qkv(sa=sa, dqkv=dqkv, xn1=xn1, dbqkv=dbqkv, dw_nq=dw_nq, dw_nk=dw_nk):
-                wg, bg, acc = sa.qkv.grads()
-                ops.gemm(dqkv, xn1, a_mn=True, b_mn=True, out=wg, accumulate=acc)
-                if acc:
-                    bg.add_(dbqkv)
-                else:
-                    bg.copy_(dbqkv)
-                _acc_vec(sa.norm_q.weight, dw_nq)
-                _acc_vec(sa.norm_k.weight, dw_nk)
-            ops.defer(wgrad_qkv)
-        dxn1 = ops.gemm(dqkv, sa.qkv.weight, b_mn=True, out=None if ops.deferring() else xn1)
-        dx, part = ops.ln_modulate_bwd(dxn1, x2, mod[:, 1], mean1, rstd1, B, L, dres=dx1, flags=ops.LN_ROUND_STEPS)
+            [{'dy': dq, 'dx': dqkva[:, 0:D], 'weight': sa.norm_q.weight, 'xhat': xhq, 'rstd': rq, 'rope': True},
+             {'dy': dk, 'dx': dqkva[:, D:2 * D], 'weight': sa.norm_k.weight, 'xhat': xhk, 'rstd': rk, 'rope': True},
+             {'dy': dv, 'dx': dqkva[:, 2 * D:3 * D]}], B, L, H, cos, sin)
+        _defer_acc((sa.norm_q.weight, dw_nq), (sa.norm_k.weight, dw_nk))
+        s_qkv.backproject(dqkva)
+        xa = s_qkv.rebuild(kept1, B * L, dev, lambda out: ops.ln_modulate_fwd(
+            x2, mod[:, 1], mod[:, 0], B, L, eps=blk.eps, out=out, save_stats=False, flags=LN_STEPS))
+        s_qkv.queue_grads(xa, dqkva, ops.colsum(dqkva) if s_qkv.bias_grad else None)
+        dxn1 = ops.gemm(dqkva, s_qkv.w_dgrad, b_mn=True, out=s_qkv.dgrad_out(xa))
+        dx, part = ops.ln_modulate_bwd(dxn1, x2, mod[:, 1], mean1, rstd1, B, L, dres=dx1, flags=LN_STEPS)
         ops.colreduce_finish(part, per_sample0=dmod[:, 1], per_sample1=dmod[:, 0])
         # ---- modulation: e = modulation + e0 ----
         if blk.modulation.requires_grad:
@@ -361,6 +366,9 @@ class WanAttentionBlock(nn.Module):
         self.ffn = nn.ModuleList([_plain(ffn_dim, dim, dtype, device), nn.Identity(), _plain(dim, ffn_dim, dtype, device)])
         self.modulation = nn.Parameter(torch.randn(1, 6, dim, device=device).to(dtype) / dim ** 0.5)
         self.__dict__['_ones_cache'] = {}
+        sa, ca = self.self_attn, self.cross_attn
+        self.sites = {'sa_qkv': DenseSite(sa.qkv), 'sa_o': DenseSite(sa.o), 'ca_q': DenseSite(ca.q), 'ca_kv': DenseSite(ca.kv),
+                      'ca_o': DenseSite(ca.o), 'ffn1': DenseSite(self.ffn[0]), 'ffn2': DenseSite(self.ffn[2])}
 
     def _ones(self, B, D, device):
         key = (B, D, str(device))
@@ -371,9 +379,6 @@ class WanAttentionBlock(nn.Module):
 
     def forward(self, x, e, seq_lens, grid_sizes, freqs, context, context_lens=None):
         assert context_lens is None, 'the reference passes context_lens=None (models/wan/wan.py:526)'
-        if 'lora' in self.__dict__:          # adapters attached (lora.py): frozen base, K-extended GEMMs
-            from .lora import WanBlockLoraFn
-            return WanBlockLoraFn.apply(self, x, e, context, freqs[0], freqs[1])
         return WanBlockFn.apply(self, x, e, context, freqs[0], freqs[1])
 
 

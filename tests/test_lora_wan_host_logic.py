@@ -1,4 +1,4 @@
-"""CPU: LoRA on the Wan attention block (lora.py: WanBlockLoraFn) on the kernel test doubles against the oracle with
+"""CPU: LoRA on the Wan attention block (wan.WanBlockFn over lora.LoraSite sites) on the kernel test doubles against the oracle with
 PEFT-style adapters; the real kernels are exercised by tests/test_wan_gpu.py::test_wan_lora_matches_oracle."""
 import os
 import sys
