@@ -127,6 +127,9 @@ SIGNATURES['dpipe_adamw_step'] = (c_int, [c_void_p, c_void_p, c_void_p, c_void_p
 SIGNATURES['dpipe_automagic_scratch_doubles'] = (c_int, [c_void_p, c_int, ctypes.POINTER(c_int64)])
 SIGNATURES['dpipe_automagic_stats'] = (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p])
 SIGNATURES['dpipe_automagic_apply'] = (c_int, [c_void_p, c_int, c_void_p, c_void_p])
+SIGNATURES['dpipe_prodigy_scratch_doubles'] = (c_int, [c_void_p, c_int, ctypes.POINTER(c_int64)])
+SIGNATURES['dpipe_prodigy_stats'] = (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int64, c_void_p])
+SIGNATURES['dpipe_prodigy_apply'] = (c_int, [c_void_p, c_int, c_void_p, c_void_p])
 SIGNATURES['dpipe_noise_pack'] = (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int64, c_int, c_int,
                                           c_int, c_void_p])
 SIGNATURES['dpipe_exec_create'] = (c_int, [c_int, c_int, ctypes.c_double, ctypes.POINTER(c_void_p)])
@@ -152,3 +155,20 @@ class AutomagicScalars(ctypes.Structure):
     _fields_ = [('beta2', ctypes.c_double), ('eps', ctypes.c_double), ('lr_bump', ctypes.c_double),
                 ('min_lr', ctypes.c_double), ('max_lr', ctypes.c_double), ('clip_threshold', ctypes.c_double),
                 ('weight_decay', ctypes.c_double)]
+
+
+class ProdigyTensor(ctypes.Structure):
+    _fields_ = [('p', c_void_p), ('g', c_void_p), ('p0', c_void_p), ('s', c_void_p), ('m', c_void_p), ('v', c_void_p),
+                ('numel', c_int64), ('weight_decay', ctypes.c_double), ('eps', ctypes.c_double), ('dtype', c_int),
+                ('fixed_decay', c_int)]
+
+
+class ProdigyScalars(ctypes.Structure):
+    _fields_ = [('lr', ctypes.c_double), ('beta1', ctypes.c_double), ('beta2', ctypes.c_double),
+                ('beta3', ctypes.c_double), ('d0', ctypes.c_double), ('d_coef', ctypes.c_double),
+                ('growth_rate', ctypes.c_double), ('bias_correction', c_int), ('safeguard_warmup', c_int)]
+
+
+# slots of the Prodigy device scalar block (include/dpipe.h DPIPE_PRODIGY_*)
+PRODIGY_SLOTS = {'d': 0, 'd_max': 1, 'd_hat': 2, 'd_numerator': 3, 'd_denom': 4, 'step': 5, 'd_lr': 6, 'skip': 7}
+PRODIGY_STATE_DOUBLES = 8

@@ -1,6 +1,7 @@
 """Tensor-level wrappers over the C ABI (include/dpipe.h).  torch is used only for device memory and streams;
 every compute call goes to libdpipe_b200.so, and a missing library raises (no fallback)."""
 import ctypes
+import math
 
 import torch
 
@@ -681,6 +682,96 @@ def automagic_apply(params, grads, rows, cols, vs, codes, scales, polarities, sh
     # the kernel wrote the weights behind autograd's back: move their version counters as an in-place op would, so
     # that caches keyed on them (lora.py's fused factor buffers) see the new values
     for p in params:
+        torch.autograd.graph.increment_version(p)
+
+
+class ProdigyArgs:
+    """The packed per-tensor arguments of Prodigy steps (include/dpipe.h dpipe_prodigy_tensor) and their fp64 scratch,
+    built once by `prodigy_pack` and reused while the parameters, their state and the group options stay the same:
+    filling the ctypes array costs host time per tensor.  It holds no gradients: `prodigy_stats` writes the gradient
+    pointers of each step into the packed array with one tensor copy and keeps no reference to them.
+    scratch[2i], scratch[2i + 1] hold tensor i's dot(g, p0 - p) and sum(|s|) after `prodigy_stats`."""
+
+    def __init__(self, arr, params, s, p0, m, v, scratch):
+        self.arr, self.n = arr, len(params)
+        self.params, self.s, self.p0, self.m, self.v = params, s, p0, m, v
+        self.scratch = scratch
+        self.chunks = (sum(1 for p in params if p.numel()) + 63) // 64      # launches per phase (empty tensors skipped)
+        words = torch.frombuffer(arr, dtype=torch.int64).view(-1, ctypes.sizeof(_abi.ProdigyTensor) // 8)
+        self._g = words[:self.n, _abi.ProdigyTensor.g.offset // 8]          # the `g` field of every entry
+
+    def set_grads(self, grads):
+        """point the packed entries at this step's gradients (same shape, dtype, device and contiguity as the
+        parameters)"""
+        if len(grads) != self.n:
+            raise ValueError(f'prodigy: {len(grads)} gradients for {self.n} parameters')
+        for i, (p, g) in enumerate(zip(self.params, grads)):
+            if g is None or g.dtype != p.dtype or g.shape != p.shape or g.get_device() != p.get_device() \
+                    or not g.is_contiguous():
+                got = 'None' if g is None else f'{g.dtype} {tuple(g.shape)} on {g.device}'
+                raise TypeError(f'prodigy: grad {i} must be a contiguous {p.dtype} tensor of shape {tuple(p.shape)} '
+                                f'on {p.device}, got {got}')
+        if self.n:
+            self._g.copy_(torch.tensor([g.data_ptr() for g in grads], dtype=torch.int64))
+
+
+def prodigy_pack(params, s, p0, m, v, weight_decay, eps, fixed_decay, device=None):
+    """ProdigyArgs for the parameters of every param group in group order: per parameter its state tensors s, p0,
+    exp_avg (m), exp_avg_sq (v) (contiguous CUDA tensors of its shape and dtype, bf16 or fp32) and its group's
+    weight_decay, eps, fixed_decay.  device: where the scratch goes (the parameters' device by default)."""
+    n = len(params)
+    if any(len(x) != n for x in (s, p0, m, v, weight_decay, eps, fixed_decay)):
+        raise ValueError('prodigy_pack: the argument lists differ in length')
+    arr = (_abi.ProdigyTensor * max(1, n))()
+    for i, p in enumerate(params):
+        if p.dtype not in _GRAD_DTYPES:
+            raise TypeError(f'prodigy: tensor {i} is {p.dtype}; the kernels take bf16 or fp32 weights')
+        for t, name in ((p, 'param'), (s[i], 's'), (p0[i], 'p0'), (m[i], 'exp_avg'), (v[i], 'exp_avg_sq')):
+            if t is None or not t.is_cuda or t.dtype != p.dtype or t.shape != p.shape or not t.is_contiguous():
+                got = 'None' if t is None else f'{t.dtype} {tuple(t.shape)} on {t.device}'
+                raise TypeError(f'prodigy: {name} {i} must be a contiguous CUDA {p.dtype} tensor of shape '
+                                f'{tuple(p.shape)}, got {got}')
+        a = arr[i]
+        a.p, a.p0, a.s, a.m, a.v = (t.data_ptr() for t in (p, p0[i], s[i], m[i], v[i]))
+        a.g = a.p                   # a valid pointer until prodigy_stats writes the step's gradient
+        a.numel, a.weight_decay, a.eps = p.numel(), weight_decay[i], eps[i]
+        a.dtype, a.fixed_decay = _GRAD_DTYPES[p.dtype], int(bool(fixed_decay[i]))
+    need = ctypes.c_int64()
+    check(lib().dpipe_prodigy_scratch_doubles(arr, n, ctypes.byref(need)), 'dpipe_prodigy_scratch_doubles')
+    scratch = torch.empty(max(1, need.value), dtype=torch.float64, device=device if device is not None else params[0].device)
+    return ProdigyArgs(arr, list(params), list(s), list(p0), list(m), list(v), scratch)
+
+
+def prodigy_stats(args, grads, state, *, lr, betas, beta3, d0, d_coef, growth_rate, bias_correction, safeguard_warmup):
+    """Prodigy statistics phase (include/dpipe.h dpipe_prodigy_stats) over every tensor of `args` with this step's
+    gradients `grads` (one per parameter): s, exp_avg, exp_avg_sq in place; then d_numerator, d_denom, d_hat, d,
+    d_max, step and the skip flag in `state`, the optimizer's fp64 device block of _abi.PRODIGY_STATE_DOUBLES (read for
+    the old d and step).  Host scalars are group 0's hyper-parameters (beta3 None: sqrt(beta2)).  No host
+    synchronisation."""
+    global LAUNCHES
+    if state.dtype != torch.float64 or not state.is_cuda or state.numel() != _abi.PRODIGY_STATE_DOUBLES:
+        raise TypeError('prodigy_stats: state must be a CUDA fp64 tensor of '
+                        f'{_abi.PRODIGY_STATE_DOUBLES} elements')
+    args.set_grads(grads)
+    b1, b2 = betas
+    sc = _abi.ProdigyScalars(lr, b1, b2, beta3 if beta3 is not None else math.sqrt(b2), d0, d_coef, growth_rate,
+                             int(bool(bias_correction)), int(bool(safeguard_warmup)))
+    _e = _prof_begin()
+    check(lib().dpipe_prodigy_stats(args.arr, args.n, ctypes.byref(sc), state.data_ptr(), args.scratch.data_ptr(),
+                                    args.scratch.numel(), _stream()), 'dpipe_prodigy_stats')
+    _prof_end(_e, 0.0, 'prodigy_stats')
+    LAUNCHES += (1 if args.n else 0) + 2 * args.chunks + 1          # memset of the sums, stats + fold per chunk, finish
+
+
+def prodigy_apply(args, state):
+    """Prodigy apply phase (include/dpipe.h dpipe_prodigy_apply) after prodigy_stats: the weights in place, unless the
+    statistics phase set the skip flag; the weights' version counters move."""
+    global LAUNCHES
+    _e = _prof_begin()
+    check(lib().dpipe_prodigy_apply(args.arr, args.n, state.data_ptr(), _stream()), 'dpipe_prodigy_apply')
+    _prof_end(_e, 0.0, 'prodigy_apply')
+    LAUNCHES += args.chunks
+    for p in args.params:           # as automagic_apply: caches keyed on the version see the new weights
         torch.autograd.graph.increment_version(p)
 
 

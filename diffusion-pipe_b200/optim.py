@@ -12,7 +12,7 @@ import struct
 
 import torch
 
-from . import ops
+from . import _abi, ops
 
 
 def _f32(x):
@@ -271,3 +271,125 @@ step kernels refuse CPU tensors, there is no CPU path."""
             st['shift'] = (s['shift'].to(device=dev, dtype=torch.bfloat16).clone(memory_format=torch.contiguous_format) if 'shift' in s else
                            torch.zeros_like(p, memory_format=torch.contiguous_format))
         return st
+
+
+_PRODIGY_SCALARS = ('step', 'd', 'd_max', 'd_hat', 'd_numerator', 'd_denom')
+
+
+class Prodigy(torch.optim.Optimizer):
+    """pytorch_optimizer's Prodigy (`type = 'Prodigy'`, the reference's fallback `getattr(pytorch_optimizer, type)`,
+    train.py:698-700): Adam whose step size d is estimated from the run itself, so `lr = 1` needs no tuning.  Each step
+    is two fused phases over the parameters of all groups (`ops.prodigy_stats`, then `ops.prodigy_apply`;
+    csrc/prodigy.cu), with no host synchronisation: d and its statistics live in one fp64 device block.
+
+    As in the reference: d, d0, d_max, d_coef, growth_rate, lr, betas, beta3 and bias_correction come from
+    param_groups[0], and the numerator and denominator of d sum over every group, so the factory's weight-decay / no-
+    weight-decay groups share one d; weight_decay, fixed_decay and eps are read per group.  A step in which every
+    gradient is zero (d_denom == 0) updates m, v, s and d_numerator and leaves the weights, d and the step count alone.
+    `group['lr']` is read every step (LR schedulers work).
+
+    The group entries `step`, `d`, `d_max`, `d_hat`, `d_numerator` and `d_denom` carry the reference's names; during
+    training they are 0-dim views of the device block (the same in every group).  state_dict() writes them as Python
+    numbers (one sync, at save time only); load_state_dict() takes numbers or tensors.  State per parameter, allocated
+    like the parameter: `s`, `p0`, `exp_avg`, `exp_avg_sq` (8 B per bf16 parameter), no Kahan summation (the
+    reference's optimizer has none).  Only decoupled weight decay; bf16 / fp32 parameters on a CUDA device (fp16, fp8
+    and CPU tensors are refused)."""
+
+    def __init__(self, params, lr=1.0, betas=(0.9, 0.999), beta3=None, d0=1e-6, d_coef=1.0, growth_rate=float('inf'),
+                 weight_decay=0.0, weight_decouple=True, fixed_decay=False, bias_correction=False,
+                 safeguard_warmup=False, eps=1e-8, gradient_release=False):
+        if gradient_release:
+            raise NotImplementedError('prodigy: gradient_release is not supported (d is estimated from every '
+                                      'parameter before any weight moves)')
+        if not weight_decouple:
+            raise NotImplementedError('prodigy: weight_decouple=False (L2 weight decay added to the gradient) is not '
+                                      'supported; decoupled weight decay is')
+        if not 0.0 <= lr:
+            raise ValueError(f'invalid learning rate {lr}')
+        if not (0.0 <= betas[0] < 1.0 and 0.0 <= betas[1] < 1.0):
+            raise ValueError(f'invalid betas {betas}')
+        if not d0 > 0.0:
+            raise ValueError(f'invalid d0 {d0}')
+        if not 0.0 <= weight_decay:
+            raise ValueError(f'invalid weight_decay {weight_decay}')
+        if not 0.0 <= eps:
+            raise ValueError(f'invalid eps {eps}')
+        defaults = dict(lr=lr, betas=tuple(betas), beta3=beta3, d0=d0, d_coef=d_coef, growth_rate=growth_rate,
+                        weight_decay=weight_decay, weight_decouple=True, fixed_decay=fixed_decay,
+                        bias_correction=bias_correction, safeguard_warmup=safeguard_warmup, eps=eps)
+        super().__init__(params, defaults)
+        dev = None
+        for group in self.param_groups:
+            for p in group['params']:
+                if p.dtype not in (torch.bfloat16, torch.float32):
+                    raise TypeError(f'prodigy: parameters must be bf16 or fp32 tensors, got {p.dtype}')
+                dev = dev or p.device
+        self._block = torch.zeros(_abi.PRODIGY_STATE_DOUBLES, dtype=torch.float64, device=dev)
+        self._set_block({})
+        self._packed = (None, None)
+
+    def _set_block(self, values):
+        """write the group scalars (numbers or tensors) into the device block, and point every group's entries at it;
+        d, d_max and d_hat default to d0, the others to 0"""
+        d0 = self.param_groups[0]['d0']
+        vals = [0.0] * _abi.PRODIGY_STATE_DOUBLES
+        for k, v in dict({'d': d0, 'd_max': d0, 'd_hat': d0}, **values).items():
+            vals[_abi.PRODIGY_SLOTS[k]] = float(v)
+        self._block.copy_(torch.tensor(vals, dtype=torch.float64))
+        for group in self.param_groups:
+            for k in _PRODIGY_SCALARS:
+                group[k] = self._block[_abi.PRODIGY_SLOTS[k]]
+
+    def mean_d(self):
+        """the mean of the groups' d as a device scalar (no sync), what the reference logs as train/prodigy_d"""
+        return torch.stack([g['d'] for g in self.param_groups]).mean()
+
+    def _init_state(self, p):
+        state = self.state[p]
+        state['s'] = torch.zeros_like(p, memory_format=torch.contiguous_format)
+        state['p0'] = p.detach().clone(memory_format=torch.contiguous_format)
+        state['exp_avg'] = torch.zeros_like(p, memory_format=torch.contiguous_format)
+        state['exp_avg_sq'] = torch.zeros_like(p, memory_format=torch.contiguous_format)
+        return state
+
+    def _args(self, ps):
+        """ops.ProdigyArgs for the (parameter, group) pairs ps, rebuilt only when that list, a parameter's storage or a
+        group's weight_decay / eps / fixed_decay changes (the gradients are passed to each step, not packed)"""
+        key = tuple((id(p), p.data_ptr(), g['weight_decay'], g['eps'], g['fixed_decay']) for p, g in ps)
+        if self._packed[0] != key:
+            sts = [self.state[p] if self.state[p] else self._init_state(p) for p, _ in ps]
+            self._packed = (key, ops.prodigy_pack(
+                [p for p, _ in ps], [s['s'] for s in sts], [s['p0'] for s in sts], [s['exp_avg'] for s in sts],
+                [s['exp_avg_sq'] for s in sts], [g['weight_decay'] for _, g in ps], [g['eps'] for _, g in ps],
+                [g['fixed_decay'] for _, g in ps], device=self._block.device))
+        return self._packed[1]
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        ps = [(p, group) for group in self.param_groups for p in group['params'] if p.grad is not None]
+        args = self._args(ps)
+        g0 = self.param_groups[0]
+        ops.prodigy_stats(args, [p.grad for p, _ in ps], self._block, lr=g0['lr'], betas=g0['betas'],
+                          beta3=g0['beta3'], d0=g0['d0'], d_coef=g0['d_coef'], growth_rate=g0['growth_rate'],
+                          bias_correction=g0['bias_correction'], safeguard_warmup=g0['safeguard_warmup'])
+        ops.prodigy_apply(args, self._block)
+        return loss
+
+    def state_dict(self):
+        sd = super().state_dict()
+        vals = self._block.tolist()                              # the one sync, at save time
+        for g in sd['param_groups']:
+            for k in _PRODIGY_SCALARS:
+                g[k] = vals[_abi.PRODIGY_SLOTS[k]]
+            g['step'] = int(g['step'])
+        return sd
+
+    def load_state_dict(self, state_dict):
+        super().load_state_dict(state_dict)
+        g0 = self.param_groups[0]
+        self._set_block({k: g0[k] for k in _PRODIGY_SCALARS if k in g0})
+        self._packed = (None, None)

@@ -313,6 +313,63 @@ int dpipe_automagic_stats(const dpipe_automagic_tensor* t, int n, const dpipe_au
  * torch op rounds: bit-identical to oracle/automagic_ref.py automagic_apply_emulated.
  * replaces: the update half of Automagic.step (optimizers/automagic.py:300-344). */
 int dpipe_automagic_apply(const dpipe_automagic_tensor* t, int n, const dpipe_automagic_scalars* s, void* stream);
+/* One parameter of a Prodigy step (pytorch_optimizer.Prodigy, built for `type = 'Prodigy'`).  p, g and the state s, p0,
+ * m = exp_avg, v = exp_avg_sq: numel elements each of dtype (0 = bf16, 1 = fp32), contiguous, at any element offset
+ * (16-byte vectors when all six share their offset mod 16 B).  weight_decay (decoupled), fixed_decay and eps are the
+ * parameter's group's. */
+typedef struct dpipe_prodigy_tensor {
+    void* p;
+    const void* g;
+    const void* p0;
+    void* s;
+    void* m;
+    void* v;
+    int64_t numel;
+    double weight_decay;
+    double eps;
+    int dtype;
+    int fixed_decay;
+} dpipe_prodigy_tensor;
+/* group 0's hyper-parameters, as the Python floats the reference passes (beta3: sqrt(beta2) when it is None) */
+typedef struct dpipe_prodigy_scalars {
+    double lr, beta1, beta2, beta3, d0, d_coef, growth_rate;
+    int bias_correction, safeguard_warmup;
+} dpipe_prodigy_scalars;
+/* the optimizer's device scalar block (fp64), shared by all its param groups, read and written only by the kernels */
+#define DPIPE_PRODIGY_D 0
+#define DPIPE_PRODIGY_D_MAX 1
+#define DPIPE_PRODIGY_D_HAT 2
+#define DPIPE_PRODIGY_D_NUMERATOR 3
+#define DPIPE_PRODIGY_D_DENOM 4
+#define DPIPE_PRODIGY_STEP 5
+#define DPIPE_PRODIGY_D_LR 6 /* d * lr / bias_correction of the last statistics phase (its old d) */
+#define DPIPE_PRODIGY_SKIP 7 /* 1 when the last statistics phase found d_denom == 0 */
+#define DPIPE_PRODIGY_STATE_DOUBLES 8
+/* doubles of fp64 scratch dpipe_prodigy_stats needs: 2 * n per-tensor sums, then the per-CTA partials of the largest
+ * chunk of 64 */
+int dpipe_prodigy_scratch_doubles(const dpipe_prodigy_tensor* t, int n, int64_t* out);
+/* Prodigy statistics phase over the n parameters of ALL param groups in group order, 64 per launch (2 launches per 64,
+ * then 1), no host synchronisation.  From the device block (old d, step) and the host scalars, in double:
+ *   t = step + 1, bc = (1 - beta1^t) / sqrt(1 - beta2^t) (powers by squaring; 1 without bias_correction),
+ *   d_lr = d * lr / bc, k = (d / d0) * d_lr; per element in fp32 (coefficients rounded to fp32):
+ *   m = fma(g, d * (1 - beta1), m * beta1);  v = fma(d * d * (1 - beta2), g * g, v * beta2);
+ *   s = fma(g, (d / d0) * (safeguard_warmup ? d : d_lr), s * beta3)      (rounded to bf16 after each op for bf16)
+ *   per tensor in fp64: dot_i = sum g * (p0 - p), abs_i = sum |s| (per-CTA partials, fixed-order folds: bitwise
+ *   repeatable, no float atomics), written to scratch[2i], scratch[2i + 1];
+ *   then one CTA, in tensor order: d_numerator = beta3 * d_numerator + k * dot_0 + k * dot_1 ..., d_denom = sum abs_i;
+ *   d_denom == 0: SKIP = 1 (d, d_max, d_hat and step unchanged); otherwise d_hat = d_coef * d_numerator / d_denom,
+ *   d = max(d, d_hat) if d == d0, d_max = max(d_max, d_hat), d = min(d_max, d * growth_rate), step = t, SKIP = 0.
+ * Empty tensors are skipped (their sums are 0).  Bit-identical to oracle/prodigy_ref.py prodigy_stats_emulated /
+ * prodigy_fold, whose elementwise order is that of torch's CUDA kernels.
+ * replaces: the first loop of Prodigy.step and its d_denom / d_hat host syncs (train.py:698-700). */
+int dpipe_prodigy_stats(const dpipe_prodigy_tensor* t, int n, const dpipe_prodigy_scalars* s, double* state,
+                        double* scratch, int64_t scratch_len, void* stream);
+/* Prodigy apply phase after dpipe_prodigy_stats (any subset of its tensors), one launch per 64; returns at once on
+ * the device when SKIP is set.  With the old d_lr and the new d from the block, per element in fp32:
+ *   denom = sqrt(v) + d * eps;  p = p * (1 - weight_decay * (fixed_decay ? 1 : d_lr));  p = fma(-d_lr, m / denom, p)
+ * (rounded to bf16 after each op for bf16).  Bit-identical to oracle/prodigy_ref.py prodigy_apply_emulated.
+ * replaces: the second loop of Prodigy.step (train.py:698-700). */
+int dpipe_prodigy_apply(const dpipe_prodigy_tensor* t, int n, const double* state, void* stream);
 /* flow-matching noising of one batch on the device, fp32, IEEE-rounded multiplies and adds (bit-identical to the host ops):
  *   xt = (1 - t[b]) * x1 + t[b] * x0,   target = x0 - x1      x1, x0: [bs, c, frames, h, w] contiguous; t: [bs]
  * pack != 0 (frames == 1): both outputs in diffusers' packed layout [bs, (h/2)(w/2), 4c] (2x2 patches, channel-major).

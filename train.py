@@ -7,8 +7,10 @@ Same CLI flags and TOML keys as the reference for everything on the hot path (SU
 `pipeline_stages`, `micro_batch_size_per_gpu` (int or [[res, bs], ...]), `gradient_accumulation_steps`,
 `gradient_clipping`, `partition_method` / `partition_split`, `[optimizer]` (type adamw = torch's fused AdamW, adamw_optimi =
 optimi's AdamW with Kahan-summed bf16 weights on the fused step kernel, automagic = the reference's Automagic on its
-fused step kernels, sgd; `betas`, `weight_decay`, `eps`, `lr`, `kahan_sum`, `decouple_lr`, `max_lr`; automagic:
-`min_lr`, `max_lr`, `lr_bump`, `clip_threshold`, `beta2`), `lr_scheduler`, `warmup_steps`, `epochs`, `max_steps`, `save_every_n_*`,
+fused step kernels, prodigy = pytorch_optimizer's Prodigy on its fused step kernels with d kept on the device, sgd;
+`betas`, `weight_decay`, `eps`, `lr`, `kahan_sum`, `decouple_lr`, `max_lr`; automagic: `min_lr`, `max_lr`, `lr_bump`,
+`clip_threshold`, `beta2`; prodigy: `beta3`, `d0`, `d_coef`, `growth_rate`, `fixed_decay`, `bias_correction`,
+`safeguard_warmup`; `train/prodigy_d` is logged with the loss), `lr_scheduler`, `warmup_steps`, `epochs`, `max_steps`, `save_every_n_*`,
 `checkpoint_every_n_minutes`, `--resume_from_checkpoint`, `--reset_dataloader`, `--reset_optimizer`.
 
 What is deliberately NOT here (out of the hot path, SURVEY.md section 8): VAE / text-encoder caching of a raw image
@@ -266,6 +268,9 @@ def make_optimizer_factory(config, model, global_batch_size=1):
         if typ == 'automagic':                          # optimizers/automagic.py (train.py:692-694): fused step kernels
             from diffusion_pipe_b200 import optim
             return optim.Automagic(groups, **oc)
+        if typ == 'prodigy':                            # pytorch_optimizer.Prodigy (train.py:698-700): fused step kernels
+            from diffusion_pipe_b200 import optim
+            return optim.Prodigy(groups, gradient_release=config['optimizer'].get('gradient_release', False), **oc)
         if typ == 'sgd':
             return torch.optim.SGD(groups, **oc)
         raise NotImplementedError(f'optimizer type {typ} is not wired into this driver (third-party optimizers are out of '
@@ -524,6 +529,8 @@ def main(argv=None):
             scalars.push('train/loss', loss, x_axis)
             if model_engine._grad_norm is not None:
                 scalars.push('train/grad_norm', model_engine._grad_norm, x_axis)
+            if type(optimizer).__name__ == 'Prodigy':                   # train.py:936-938, d read without a sync
+                scalars.push('train/prodigy_d', optimizer.mean_d(), x_axis)
         if (config['eval_every_n_steps'] and step % config['eval_every_n_steps'] == 0) or \
                 (finished_epoch and config['eval_every_n_epochs'] and epoch % config['eval_every_n_epochs'] == 0):
             scalars.flush(keep=0)
