@@ -3,7 +3,7 @@
 // These are rank-`batch` problems (M = batch): 113 MB of weights are streamed once per call, so they are HBM-bound and do
 // not belong on the tensor-core GEMM (a 128-row MMA tile would be >99% padding).  Forward: one warp per output row.
 // Backward: ONE pass over W and dW with one thread per 8 columns — it forms dW (+)= dmod^T · silu(temb), d bias and the
-// per-CTA partials of d silu = dmod · W; a finish kernel folds the partials through silu' into d temb.
+// per-row-chunk partials of d silu = dmod · W; a finish kernel folds the partials through silu' into d temb.
 //
 // Replaces nn.Linear(SiLU(temb)) inside diffusers AdaLayerNormZero / AdaLayerNormZeroSingle / AdaLayerNormContinuous
 // (reference call sites models/flux.py:502,525,547) and its autograd backward.
@@ -14,6 +14,8 @@ namespace dpipe {
 
 constexpr int MOD_MAX_B = 8;
 constexpr int MOD_ROWS = 64;   // weight rows per CTA in the backward pass
+constexpr int MOD_BWD_THREADS = 128;   // columns / 8 per CTA in the backward pass: 128 x 165 registers (<8>) fit any SM
+constexpr int MOD_MAX_K = 8192;
 
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + __expf(-x)); }
 __device__ __forceinline__ float silu_grad_f(float x) {
@@ -62,18 +64,31 @@ __global__ void mod_fwd_kernel(const __nv_bfloat16* __restrict__ temb, const __n
   }
 }
 
-// grid = N / MOD_ROWS CTAs of K/8 threads; thread t owns columns [8t, 8t+8)
+// grid (N / MOD_ROWS row chunks, K / (8 * MOD_BWD_THREADS) column blocks) of MOD_BWD_THREADS threads; thread t of
+// column block y owns columns [8 (y * MOD_BWD_THREADS + t), +8).  The CTA size does not depend on K, so the register
+// budget of every BMAX holds at every width.  Each output element sees the same operations in the same order whatever
+// the split.
 template <int BMAX>
-__global__ void mod_bwd_kernel(const float* __restrict__ dmod, int64_t ldd, const __nv_bfloat16* __restrict__ temb,
-                               const __nv_bfloat16* __restrict__ W, __nv_bfloat16* __restrict__ dW, int accumulate,
-                               float* __restrict__ dbias, float* __restrict__ partials, int B, int N, int K) {
+__global__ void __launch_bounds__(MOD_BWD_THREADS)
+mod_bwd_kernel(const float* __restrict__ dmod, int64_t ldd, const __nv_bfloat16* __restrict__ temb,
+               const __nv_bfloat16* __restrict__ W, __nv_bfloat16* __restrict__ dW, int accumulate,
+               float* __restrict__ dbias, float* __restrict__ partials, int B, int N, int K) {
   __shared__ float dm[BMAX][MOD_ROWS];
   const int n0 = blockIdx.x * MOD_ROWS;
   for (int i = threadIdx.x; i < B * MOD_ROWS; i += blockDim.x) {
     const int b = i / MOD_ROWS, r = i % MOD_ROWS;
     dm[b][r] = (n0 + r < N) ? bf16_round(dmod[(int64_t)b * ldd + n0 + r]) : 0.f;   // the reference's grad is a bf16 tensor
   }
-  const int col = threadIdx.x * 8;
+  __syncthreads();
+  if (dbias && blockIdx.y == 0) {   // one column block per row chunk writes d bias
+    for (int r = threadIdx.x; r < MOD_ROWS && n0 + r < N; r += blockDim.x) {
+      float v = 0.f;
+      for (int b = 0; b < B; ++b) v += dm[b][r];
+      dbias[n0 + r] = v;
+    }
+  }
+  const int col = (blockIdx.y * blockDim.x + threadIdx.x) * 8;
+  if (col >= K) return;
   float s[BMAX][8], acc[BMAX][8];
 #pragma unroll
   for (int b = 0; b < BMAX; ++b) {
@@ -82,14 +97,6 @@ __global__ void mod_bwd_kernel(const float* __restrict__ dmod, int64_t ldd, cons
       unpack8f(*reinterpret_cast<const uint4*>(temb + (int64_t)b * K + col), t);
 #pragma unroll
       for (int j = 0; j < 8; ++j) { s[b][j] = bf16_round(silu_f(t[j])); acc[b][j] = 0.f; }
-    }
-  }
-  __syncthreads();
-  if (dbias) {
-    for (int r = threadIdx.x; r < MOD_ROWS && n0 + r < N; r += blockDim.x) {   // blockDim may be smaller than MOD_ROWS
-      float v = 0.f;
-      for (int b = 0; b < B; ++b) v += dm[b][r];
-      dbias[n0 + r] = v;
     }
   }
   const int rows = min(MOD_ROWS, N - n0);
@@ -173,18 +180,18 @@ extern "C" int dpipe_mod_bwd_chunks(int N) { return (N + MOD_ROWS - 1) / MOD_ROW
 
 extern "C" int dpipe_mod_bwd(const float* dmod, int64_t ldd, const void* temb, const void* W, void* dW, int accumulate,
                              float* dbias, float* partials, float* dtemb, int B, int N, int K, void* stream) {
-  if (!dmod || !temb || !W || !partials || !dtemb || B < 1 || B > MOD_MAX_B || K % 256 || K / 8 > 1024)
-    return fail(DPIPE_EINVAL, "dpipe_mod_bwd: bad arguments (B=%d N=%d K=%d)", B, N, K);
-  if (B > 4 && K > 3328)   // mod_bwd_kernel<8>: 155 registers x K/8 threads must fit the register file
-    return fail(DPIPE_EINVAL, "dpipe_mod_bwd: batch %d with K=%d is not supported (batch <= 4 for K > 3328)", B, K);
+  if (!dmod || !temb || !W || !partials || !dtemb || B < 1 || B > MOD_MAX_B || K < 256 || K % 256 || K > MOD_MAX_K || N < 1)
+    return fail(DPIPE_EINVAL, "dpipe_mod_bwd: bad arguments (B=%d N=%d K=%d; 1 <= B <= %d, K a multiple of 256 and <= %d)", B, N,
+                K, MOD_MAX_B, MOD_MAX_K);
   const int nchunk = dpipe_mod_bwd_chunks(N);
   cudaStream_t s = (cudaStream_t)stream;
+  const dim3 grid(nchunk, (K / 8 + MOD_BWD_THREADS - 1) / MOD_BWD_THREADS);
   if (B <= 2)
-    mod_bwd_kernel<2><<<nchunk, K / 8, 0, s>>>(dmod, ldd, (const bf16*)temb, (const bf16*)W, (bf16*)dW, accumulate, dbias, partials, B, N, K);
+    mod_bwd_kernel<2><<<grid, MOD_BWD_THREADS, 0, s>>>(dmod, ldd, (const bf16*)temb, (const bf16*)W, (bf16*)dW, accumulate, dbias, partials, B, N, K);
   else if (B <= 4)
-    mod_bwd_kernel<4><<<nchunk, K / 8, 0, s>>>(dmod, ldd, (const bf16*)temb, (const bf16*)W, (bf16*)dW, accumulate, dbias, partials, B, N, K);
+    mod_bwd_kernel<4><<<grid, MOD_BWD_THREADS, 0, s>>>(dmod, ldd, (const bf16*)temb, (const bf16*)W, (bf16*)dW, accumulate, dbias, partials, B, N, K);
   else
-    mod_bwd_kernel<8><<<nchunk, K / 8, 0, s>>>(dmod, ldd, (const bf16*)temb, (const bf16*)W, (bf16*)dW, accumulate, dbias, partials, B, N, K);
+    mod_bwd_kernel<8><<<grid, MOD_BWD_THREADS, 0, s>>>(dmod, ldd, (const bf16*)temb, (const bf16*)W, (bf16*)dW, accumulate, dbias, partials, B, N, K);
   DPIPE_CUDA_CHECK(cudaGetLastError());
   mod_bwd_finish_kernel<<<dim3((K + 31) / 32, B), 256, 0, s>>>(partials, nchunk, (const bf16*)temb, dtemb, B, K);
   DPIPE_CUDA_CHECK(cudaGetLastError());

@@ -222,7 +222,9 @@ int dpipe_wan_norm_rope_bwd(const dpipe_wan_norm_bwd_args* args, void* stream);
  *   (models/flux.py:502,525,547). */
 int dpipe_mod_fwd(const void* temb, const void* W, const void* bias, void* out, int B, int N, int K, void* stream);
 /* its backward in one pass over W/dW: dW (+)= bf16(dmod)^T silu(temb); dbias[n] = sum_b dmod[b,n] (overwritten);
- * dtemb[b,:] += silu'(temb) * (dmod W).  partials: dpipe_mod_bwd_chunks(N) * B * K floats.  dW may be NULL. */
+ * dtemb[b,:] += silu'(temb) * bf16(bf16(dmod) W).  partials: dpipe_mod_bwd_chunks(N) * B * K floats.  dW and dbias may be
+ * NULL.  1 <= B <= 8 and K a multiple of 256 up to 8192, every B at every such K (fixed-size CTAs over 64-row chunks x
+ * 1024-column blocks). */
 int dpipe_mod_bwd_chunks(int N);
 int dpipe_mod_bwd(const float* dmod, int64_t ldd, const void* temb, const void* W, void* dW, int accumulate, float* dbias,
                   float* partials, float* dtemb, int B, int N, int K, void* stream);

@@ -68,7 +68,9 @@ def test_header_compiles_as_plain_c():
                                     ctypes.sizeof(_abi.QkBwdArgs), 12]
 
 
-def test_new_entry_points_validate_their_arguments_without_a_gpu():
+def test_entry_points_refuse_bad_arguments_before_any_cuda_call():
+    """Wan RMSNorm, LayerNorm, zero-bubble planner and modulation backward: out-of-range shapes fail in the host check,
+    so none of these calls (fake pointers) reaches the device"""
     lib = _lib.lib()
     assert lib.dpipe_wan_norm_rope_fwd(None, None) < 0 and b'null' in lib.dpipe_last_error()
     a = _abi.WanNormFwdArgs()
@@ -86,9 +88,10 @@ def test_new_entry_points_validate_their_arguments_without_a_gpu():
     w = (ctypes.c_int * 2)(3, 0)
     assert lib.dpipe_sched_zb_ex(4, 2, 0, 13, 17, 10, 4, w, None, 0) < 0
     assert lib.dpipe_sched_zb_makespan_ex(4, 2, 13, 17, 10, 4, w) < 0
-    # the batch-row modulation backward refuses what its register budget cannot hold
-    assert lib.dpipe_mod_bwd(buf, 0, buf, buf, buf, 0, buf, buf, buf, 8, 1024, 5120, None) < 0
-    assert b'not supported' in lib.dpipe_last_error()
+    # the batch-row modulation backward takes 1..8 samples and widths that are multiples of 256 up to 8192
+    for B, K in ((9, 5120), (0, 5120), (8, 100), (8, 8448)):
+        assert lib.dpipe_mod_bwd(buf, 0, buf, buf, buf, 0, buf, buf, buf, B, 1024, K, None) < 0, (B, K)
+        assert b'dpipe_mod_bwd: bad arguments' in lib.dpipe_last_error()
 
 
 def test_fp8_code_tables_are_torchs_widening_for_all_256_codes():

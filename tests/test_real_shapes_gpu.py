@@ -102,7 +102,7 @@ def _flux_rope(Lt, side):
     return R.flux_rope_tables(ids)
 
 
-def check_flux(kind, D, H, Lt, side, dev='cuda'):
+def check_flux(kind, D, H, Lt, side, dev='cuda', batch=1):
     from diffusion_pipe_b200 import flux_blocks as FB
     from oracle import flux_ref as R
     Li = side * side
@@ -115,9 +115,9 @@ def check_flux(kind, D, H, Lt, side, dev='cuda'):
     _load(ref, blk)
     cos, sin = _flux_rope(Lt, side)
     g = torch.Generator().manual_seed(3)
-    hid, enc = torch.randn(1, Li, D, generator=g).bfloat16(), torch.randn(1, Lt, D, generator=g).bfloat16()
-    temb = torch.randn(1, D, generator=g).bfloat16()
-    t_h, t_e = torch.randn(1, Li, D, generator=g).bfloat16(), torch.randn(1, Lt, D, generator=g).bfloat16()
+    hid, enc = torch.randn(batch, Li, D, generator=g).bfloat16(), torch.randn(batch, Lt, D, generator=g).bfloat16()
+    temb = torch.randn(batch, D, generator=g).bfloat16()   # a different modulation row per sample
+    t_h, t_e = torch.randn(batch, Li, D, generator=g).bfloat16(), torch.randn(batch, Lt, D, generator=g).bfloat16()
 
     def run(block, dev, dtype):
         h = hid.detach().clone().to(dev, dtype).requires_grad_(True)
@@ -137,7 +137,14 @@ def test_flux_dev_block_at_1024px(kind):
     check_flux(kind, D=3072, H=24, Lt=512, side=64)
 
 
-def check_qwen(D, H, Lt, side, dev='cuda'):
+@pytest.mark.parametrize('kind', ['double', 'single'])
+def test_flux_block_at_micro_batch_3(kind):
+    """three samples with their own temb at the Flux width and head count, short sequence: the per-sample gate of
+    EPI_GATE_RES, the batch index of the QKV epilogue and the 3-4 sample modulation backward inside real blocks"""
+    check_flux(kind, D=3072, H=24, Lt=128, side=32, batch=3)
+
+
+def check_qwen(D, H, Lt, side, dev='cuda', batch=1):
     from diffusion_pipe_b200 import qwen_image as QI
     from oracle import qwen_ref as Q
     Li = side * side
@@ -149,9 +156,9 @@ def check_qwen(D, H, Lt, side, dev='cuda'):
     vid, txt = torch.stack([vc, vs]), torch.stack([tc, ts])          # [2, L, 128] each (cos, sin)
     joint = torch.cat([txt, vid], dim=1)
     g = torch.Generator().manual_seed(4)
-    hid, enc = torch.randn(1, Li, D, generator=g).bfloat16(), torch.randn(1, Lt, D, generator=g).bfloat16()
-    temb = torch.randn(1, D, generator=g).bfloat16()
-    t_h, t_e = torch.randn(1, Li, D, generator=g).bfloat16(), torch.randn(1, Lt, D, generator=g).bfloat16()
+    hid, enc = torch.randn(batch, Li, D, generator=g).bfloat16(), torch.randn(batch, Lt, D, generator=g).bfloat16()
+    temb = torch.randn(batch, D, generator=g).bfloat16()
+    t_h, t_e = torch.randn(batch, Li, D, generator=g).bfloat16(), torch.randn(batch, Lt, D, generator=g).bfloat16()
 
     def finish(eo, ho, h, e, t, dev):
         loss = ((ho.float() - t_h.to(dev).float()) ** 2).mean() + ((eo.float() - t_e.to(dev).float()) ** 2).mean()
@@ -174,6 +181,10 @@ def check_qwen(D, H, Lt, side, dev='cuda'):
 def test_qwen_image_block_at_1024px():
     """models/qwen_image.py:519-605 + QwenDoubleStreamAttnProcessor2_0 (:91-174): biased q/k/v, separate image / text rope"""
     check_qwen(D=3072, H=24, Lt=256, side=64)
+
+
+def test_qwen_image_block_at_micro_batch_3():
+    check_qwen(D=3072, H=24, Lt=128, side=32, batch=3)
 
 
 def check_wan(D, F, H, Lc, grid, dev='cuda'):
