@@ -130,6 +130,7 @@ SIGNATURES['dpipe_automagic_apply'] = (c_int, [c_void_p, c_int, c_void_p, c_void
 SIGNATURES['dpipe_prodigy_scratch_doubles'] = (c_int, [c_void_p, c_int, ctypes.POINTER(c_int64)])
 SIGNATURES['dpipe_prodigy_stats'] = (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int64, c_void_p])
 SIGNATURES['dpipe_prodigy_apply'] = (c_int, [c_void_p, c_int, c_void_p, c_void_p])
+SIGNATURES['dpipe_adamw8bit_step'] = (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p])
 SIGNATURES['dpipe_noise_pack'] = (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int64, c_int, c_int,
                                           c_int, c_void_p])
 SIGNATURES['dpipe_exec_create'] = (c_int, [c_int, c_int, ctypes.c_double, ctypes.POINTER(c_void_p)])
@@ -172,3 +173,9 @@ class ProdigyScalars(ctypes.Structure):
 # slots of the Prodigy device scalar block (include/dpipe.h DPIPE_PRODIGY_*)
 PRODIGY_SLOTS = {'d': 0, 'd_max': 1, 'd_hat': 2, 'd_numerator': 3, 'd_denom': 4, 'step': 5, 'd_lr': 6, 'skip': 7}
 PRODIGY_STATE_DOUBLES = 8
+
+
+class Adamw8bitTensor(ctypes.Structure):
+    _fields_ = [('p', c_void_p), ('g', c_void_p), ('state1', c_void_p), ('state2', c_void_p), ('absmax1', c_void_p),
+                ('absmax2', c_void_p), ('numel', c_int64), ('step_size', c_float), ('beta1', c_float),
+                ('beta2', c_float), ('eps_c2', c_float), ('decay', c_float), ('dtype', c_int)]

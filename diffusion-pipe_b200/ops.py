@@ -775,6 +775,79 @@ def prodigy_apply(args, state):
         torch.autograd.graph.increment_version(p)
 
 
+_A8_DTYPE = None
+
+
+def _a8_dtype():
+    global _A8_DTYPE
+    if _A8_DTYPE is None:
+        import numpy as np
+        _A8_DTYPE = np.dtype(_abi.Adamw8bitTensor)
+    return _A8_DTYPE
+
+
+def adamw8bit_step(params, grads, state1, state2, absmax1, absmax2, scalars, qmap1=None, qmap2=None):
+    """One AdamW8bit step (include/dpipe.h dpipe_adamw8bit_step) over parameter i with its gradient and state, in
+    place: state1 / state2 fp32 m / v like the parameter with absmax1[i] = absmax2[i] = None, or uint8 codes like the
+    parameter with fp32 absmax of ceil(numel / 256) blocks; scalars[i] the dict of oracle/adamw8bit_ref.py step_scalars
+    (step_size, beta1, beta2, eps_c2, decay) for its group and step.  qmap1 / qmap2: the 256-entry fp32 maps of every
+    8-bit tensor of the call.  Parameters and gradients are contiguous CUDA bf16 / fp32 tensors.  No host
+    synchronisation; the weights' version counters move."""
+    global LAUNCHES
+    n = len(params)
+    if any(len(x) != n for x in (grads, state1, state2, absmax1, absmax2, scalars)):
+        raise ValueError('adamw8bit_step: the argument lists differ in length')
+
+    def bad(what, i, t, want):
+        got = 'None' if t is None else f'{t.dtype} {tuple(t.shape)} on {t.device}'
+        return TypeError(f'adamw8bit_step: {what} {i} must be {want}, got {got}')
+    q8 = False
+    for i, p in enumerate(params):
+        if p.dtype not in _GRAD_DTYPES:
+            raise TypeError(f'adamw8bit_step: tensor {i} is {p.dtype}; the kernel takes bf16 or fp32 weights')
+        if not p.is_cuda or not p.is_contiguous():
+            raise bad('param', i, p, 'a contiguous CUDA tensor')
+        g = grads[i]
+        if g is None or g.dtype != p.dtype or g.shape != p.shape or g.device != p.device or not g.is_contiguous():
+            raise bad('grad', i, g, f'a contiguous {p.dtype} tensor of shape {tuple(p.shape)} on {p.device}')
+        a1, a2 = absmax1[i], absmax2[i]
+        sdt = torch.float32 if a1 is None else torch.uint8
+        for t, what in ((state1[i], 'state1'), (state2[i], 'state2')):
+            if t is None or t.dtype != sdt or t.numel() != p.numel() or t.device != p.device or not t.is_contiguous():
+                raise bad(what, i, t, f'a contiguous {sdt} tensor of {p.numel()} elements on {p.device}')
+        if (a1 is None) != (a2 is None):
+            raise TypeError(f'adamw8bit_step: tensor {i}: absmax1 and absmax2 are both given or both None')
+        if a1 is not None:
+            q8 = True
+            nb = (p.numel() + 255) // 256
+            for t, what in ((a1, 'absmax1'), (a2, 'absmax2')):
+                if t.dtype != torch.float32 or t.numel() != nb or t.device != p.device or not t.is_contiguous():
+                    raise bad(what, i, t, f'a contiguous fp32 tensor of {nb} elements on {p.device}')
+    if q8:
+        for t, what in ((qmap1, 'qmap1'), (qmap2, 'qmap2')):
+            if t is None or t.dtype != torch.float32 or t.numel() != 256 or t.device != params[0].device \
+                    or not t.is_contiguous():
+                raise bad(what, 0, t, f'a contiguous fp32 tensor of 256 elements on {params[0].device}')
+    if n == 0:
+        return
+    import numpy as np
+    arr = np.zeros(n, dtype=_a8_dtype())
+    for f, ts in (('p', params), ('g', grads), ('state1', state1), ('state2', state2), ('absmax1', absmax1),
+                  ('absmax2', absmax2)):
+        arr[f] = [0 if t is None else t.data_ptr() for t in ts]
+    arr['numel'] = [p.numel() for p in params]
+    for f in ('step_size', 'beta1', 'beta2', 'eps_c2', 'decay'):
+        arr[f] = [s[f] for s in scalars]
+    arr['dtype'] = [_GRAD_DTYPES[p.dtype] for p in params]
+    _e = _prof_begin()
+    check(lib().dpipe_adamw8bit_step(arr.ctypes.data, n, qmap1.data_ptr() if q8 else None,
+                                     qmap2.data_ptr() if q8 else None, _stream()), 'dpipe_adamw8bit_step')
+    _prof_end(_e, 0.0, 'adamw8bit_step')
+    LAUNCHES += (sum(1 for p in params if p.numel()) + 63) // 64
+    for p in params:                # as automagic_apply: caches keyed on the version see the new weights
+        torch.autograd.graph.increment_version(p)
+
+
 def noise_pack(x1, x0, t, pack):
     """(x_t, target) = ((1-t) x1 + t x0, x0 - x1) on the device, fp32, bit-identical to the separate host ops; x1/x0 any
     [bs, ...] shape; pack=True ([bs, c, h, w]) writes diffusers' 2x2-packed [bs, (h/2)(w/2), 4c] layout."""

@@ -8,6 +8,7 @@ weight carries a bf16 compensation buffer holding what the last rounding dropped
 State per parameter, allocated like the parameter (bf16 for bf16 weights): `step` (host int), `exp_avg`, `exp_avg_sq` and,
 with Kahan summation, `kahan_comp` — 6 B per bf16 parameter (4 B without Kahan), against 4 B for torch.optim.AdamW.
 """
+import math
 import struct
 
 import torch
@@ -393,3 +394,142 @@ class Prodigy(torch.optim.Optimizer):
         g0 = self.param_groups[0]
         self._set_block({k: g0[k] for k in _PRODIGY_SCALARS if k in g0})
         self._packed = (None, None)
+
+
+def dynamic_map(signed):
+    """bitsandbytes' create_dynamic_map(signed) (8 bits, 7 exponent bits): for each decade 10^(i-6), i = 0..6, the
+    midpoints of linspace(0.1, 1, 2^i + 1) (signed, mirrored to negative values) or of linspace(0.1, 1, 2^(i+1) + 1)
+    (unsigned), then 0 and 1.0; 256 sorted fp32 values"""
+    data = []
+    for i in range(7):
+        b = torch.linspace(0.1, 1, (2 ** i if signed else 2 ** (i + 1)) + 1, dtype=torch.float32)
+        means = (b[:-1] + b[1:]) / 2.0
+        data += ((10 ** (i - 6)) * means).tolist()
+        if signed:
+            data += (-(10 ** (i - 6)) * means).tolist()
+    data += [0.0, 1.0]
+    return torch.tensor(sorted(data), dtype=torch.float32)
+
+
+_A8_TENSORS = ('state1', 'state2', 'qmap1', 'qmap2', 'absmax1', 'absmax2')
+
+
+class AdamW8bit(torch.optim.Optimizer):
+    """bitsandbytes' AdamW8bit (`type = 'adamw8bit'`, train.py:650-700): Adam with decoupled weight decay whose moments
+    are uint8 codes of bnb's dynamic maps with one fp32 absmax per 256 elements, about 2.03 B of state per parameter
+    (adamw_optimi with Kahan: 6 B).  Parameters below `min_8bit_size` elements keep fp32 moments, as in bnb.  Every step
+    is one multi-tensor kernel launch per 64 parameters over all groups (`ops.adamw8bit_step`, csrc/adamw8bit.cu), with
+    no host synchronisation; its rule is oracle/adamw8bit_ref.py's.
+
+    bnb's constructor surface and defaults; `optim_bits` is ignored, as in bnb.  block_wise=False, percentile_clipping
+    other than 100, amsgrad, is_paged and gradient_release are refused.  `group['lr']`, betas, eps and weight_decay are
+    read on every step (LR schedulers work).  Parameters without a gradient are skipped and their step count does not
+    advance.  State per parameter, bnb's keys: `step` (int), `state1`, `state2` and, for 8-bit states, `qmap1`, `qmap2`
+    (the maps, shared by the parameters of a device), `absmax1`, `absmax2`; load_state_dict() keeps every state tensor
+    in its own dtype (torch's default would cast them to the parameter dtype).  Parameters are bf16 / fp32 CUDA tensors
+    (fp16 and fp8 are refused here, CPU tensors at the step)."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, amsgrad=False, optim_bits=32,
+                 min_8bit_size=4096, percentile_clipping=100, block_wise=True, is_paged=False, gradient_release=False):
+        for flag, what in ((not block_wise, 'block_wise=False (one absmax per tensor)'),
+                           (percentile_clipping != 100, 'percentile_clipping'), (amsgrad, 'amsgrad'),
+                           (is_paged, 'is_paged (paged states)'),
+                           (gradient_release, 'gradient_release (the step runs once after the backward pass)')):
+            if flag:
+                raise NotImplementedError(f'adamw8bit: {what} is not supported')
+        if not 0.0 <= lr:
+            raise ValueError(f'invalid learning rate {lr}')
+        if not (0.0 <= betas[0] < 1.0 and 0.0 <= betas[1] < 1.0):
+            raise ValueError(f'invalid betas {betas}')
+        if not 0.0 <= weight_decay:
+            raise ValueError(f'invalid weight_decay {weight_decay}')
+        if not 0.0 <= eps:
+            raise ValueError(f'invalid eps {eps}')
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay))
+        self.min_8bit_size = min_8bit_size
+        self._maps = {}
+        for group in self.param_groups:
+            for p in group['params']:
+                if p.dtype not in (torch.bfloat16, torch.float32):
+                    raise TypeError(f'adamw8bit: parameters must be bf16 or fp32 tensors, got {p.dtype}')
+                self._maps_on(p.device)         # copied to the device here, not in a step
+
+    def _maps_on(self, device):
+        if device not in self._maps:
+            self._maps[device] = (dynamic_map(True).to(device), dynamic_map(False).to(device))
+        return self._maps[device]
+
+    def _init_state(self, p):
+        state = self.state[p]
+        state['step'] = 0
+        if p.numel() < self.min_8bit_size:
+            state['state1'] = torch.zeros(p.shape, dtype=torch.float32, device=p.device)
+            state['state2'] = torch.zeros(p.shape, dtype=torch.float32, device=p.device)
+        else:
+            nb = (p.numel() + 255) // 256
+            state['state1'] = torch.zeros(p.shape, dtype=torch.uint8, device=p.device)
+            state['qmap1'], state['qmap2'] = self._maps_on(p.device)
+            state['state2'] = torch.zeros(p.shape, dtype=torch.uint8, device=p.device)
+            state['absmax1'] = torch.zeros(nb, dtype=torch.float32, device=p.device)
+            state['absmax2'] = torch.zeros(nb, dtype=torch.float32, device=p.device)
+        return state
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        calls = {}                  # (qmap1, qmap2) -> the parameters stepped with those maps (fp32 states: any call)
+        for group in self.param_groups:
+            sc = {}
+            for p in group['params']:
+                if p.grad is None:
+                    continue
+                st = self.state[p] if self.state[p] else self._init_state(p)
+                st['step'] += 1
+                t = st['step']
+                if t not in sc:
+                    sc[t] = adamw8bit_scalars(group['lr'], group['betas'], group['eps'], group['weight_decay'], t)
+                key = (id(st['qmap1']), id(st['qmap2'])) if 'qmap1' in st else None
+                calls.setdefault(key, []).append((p, st, sc[t]))
+        if None in calls and len(calls) > 1:
+            plain = calls.pop(None)
+            calls[next(iter(calls))] += plain
+        for items in calls.values():
+            st8 = next((st for _, st, _ in items if 'qmap1' in st), {})
+            ops.adamw8bit_step([p for p, _, _ in items], [p.grad for p, _, _ in items],
+                               [st['state1'] for _, st, _ in items], [st['state2'] for _, st, _ in items],
+                               [st.get('absmax1') for _, st, _ in items], [st.get('absmax2') for _, st, _ in items],
+                               [s for _, _, s in items], st8.get('qmap1'), st8.get('qmap2'))
+        return loss
+
+    def load_state_dict(self, state_dict):
+        """torch's load, then every state tensor again from the saved one in its own dtype on the parameter's device;
+        maps equal to this optimizer's are shared again (one launch per step; one comparison per tensor here)"""
+        super().load_state_dict(state_dict)
+        saved = state_dict['state']
+        ids = [i for g in state_dict['param_groups'] for i in g['params']]
+        params = [p for g in self.param_groups for p in g['params']]
+        for pid, p in zip(ids, params):
+            if pid not in saved:
+                continue
+            st = self.state[p]
+            for k in _A8_TENSORS:
+                if k in saved[pid]:
+                    st[k] = saved[pid][k].to(device=p.device).clone(memory_format=torch.contiguous_format)
+            st['step'] = int(saved[pid]['step'])
+            if 'qmap1' in st:
+                m1, m2 = self._maps_on(p.device)
+                if torch.equal(st['qmap1'], m1) and torch.equal(st['qmap2'], m2):
+                    st['qmap1'], st['qmap2'] = m1, m2
+
+
+def adamw8bit_scalars(lr, betas, eps, weight_decay, step):
+    """bnb's per-step scalars in double on the host, rounded to fp32 (bnb takes them with powf on the device):
+    step_size = -lr * sqrt(1 - beta2^t) / (1 - beta1^t), eps_c2 = fp32(sqrt(1 - beta2^t)) * eps and
+    decay = 1 - lr * weight_decay in fp32 arithmetic, as the kernel would compute them"""
+    b1, b2 = betas
+    c2 = math.sqrt(1.0 - b2 ** step)
+    return dict(step_size=_f32(-lr * c2 / (1.0 - b1 ** step)), beta1=_f32(b1), beta2=_f32(b2),
+                eps_c2=_f32(_f32(c2) * _f32(eps)), decay=_f32(1.0 - _f32(_f32(lr) * _f32(weight_decay))))

@@ -372,6 +372,40 @@ int dpipe_prodigy_stats(const dpipe_prodigy_tensor* t, int n, const dpipe_prodig
  * (rounded to bf16 after each op for bf16).  Bit-identical to oracle/prodigy_ref.py prodigy_apply_emulated.
  * replaces: the second loop of Prodigy.step (train.py:698-700). */
 int dpipe_prodigy_apply(const dpipe_prodigy_tensor* t, int n, const double* state, void* stream);
+/* One parameter of an AdamW8bit step (bitsandbytes.optim.AdamW8bit, built for `type = 'adamw8bit'`).  p, g: numel
+ * elements of dtype (0 = bf16, 1 = fp32), contiguous, at any element offset (16-byte vectors where aligned).
+ * absmax1 == absmax2 == NULL: state1 = m, state2 = v are fp32 [numel] (bnb's 32-bit path, numel < min_8bit_size);
+ * otherwise state1 / state2 are uint8 codes [numel] of the signed / unsigned dynamic map and absmax1 / absmax2 fp32
+ * [ceil(numel / 256)].  The scalars of the parameter's step t and group, in double on the host, rounded to fp32:
+ * step_size = -lr * sqrt(1 - beta2^t) / (1 - beta1^t), eps_c2 = fp32(sqrt(1 - beta2^t)) * eps,
+ * decay = 1 - lr * weight_decay (fp32 ops). */
+typedef struct dpipe_adamw8bit_tensor {
+    void* p;
+    const void* g;
+    void* state1;
+    void* state2;
+    float* absmax1;
+    float* absmax2;
+    int64_t numel;
+    float step_size;
+    float beta1;
+    float beta2;
+    float eps_c2;
+    float decay;
+    int dtype;
+} dpipe_adamw8bit_tensor;
+/* One AdamW8bit step over n parameters, up to 64 non-empty ones per launch (one warp per 256-element block), no host
+ * synchronisation.  qmap1 / qmap2: the 256 sorted fp32 entries of the signed / unsigned map (may be NULL when no
+ * tensor has 8-bit states).  Per element, fp32 IEEE round-to-nearest ops in this order (no FMA):
+ *   8-bit: m = qmap1[state1] * absmax1[blk], v = qmap2[state2] * absmax2[blk]  (a non-finite g: m = v = 0, p kept)
+ *   m = m * beta1 + (1 - beta1) * g;  v = v * beta2 + ((1 - beta2) * g) * g
+ *   p = p + step_size * (m / (sqrt(v) + eps_c2));  p = p * decay        (each rounded to bf16 for bf16)
+ *   8-bit: absmax1[blk] = max |m|, absmax2[blk] = max v (warp max: order-free);  state1 = the nearest qmap1 entry to
+ *   m / absmax1 (counted in fp32 midpoints (q[k] + q[k+1]) * 0.5, ties down; 0 when absmax1 == 0), moved one code
+ *   towards m's sign when the entry's sign bit differs from m's;  state2 = the nearest qmap2 entry to v / absmax2.
+ * Bit-identical to oracle/adamw8bit_ref.py adamw8bit_emulated.
+ * replaces: bitsandbytes.optim.AdamW8bit.step (train.py:650-700). */
+int dpipe_adamw8bit_step(const dpipe_adamw8bit_tensor* t, int n, const float* qmap1, const float* qmap2, void* stream);
 /* flow-matching noising of one batch on the device, fp32, IEEE-rounded multiplies and adds (bit-identical to the host ops):
  *   xt = (1 - t[b]) * x1 + t[b] * x0,   target = x0 - x1      x1, x0: [bs, c, frames, h, w] contiguous; t: [bs]
  * pack != 0 (frames == 1): both outputs in diffusers' packed layout [bs, (h/2)(w/2), 4c] (2x2 patches, channel-major).
