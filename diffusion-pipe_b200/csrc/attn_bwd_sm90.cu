@@ -352,15 +352,15 @@ extern "C" int dpipe_attn_bwd(const dpipe_attn_bwd_args* a, void* stream) {
     return fail(DPIPE_EINVAL, "dpipe_attn_bwd: null argument");
   if (a->batch <= 0 || a->heads <= 0 || a->seq_q <= 0 || a->seq_k <= 0) return fail(DPIPE_EINVAL, "dpipe_attn_bwd: empty problem");
   if (a->ldo % 8 || a->lddo % 8) return fail(DPIPE_EINVAL, "dpipe_attn_bwd: ldo/lddo must be multiples of 8");
+  // o and d_o are read 4 bf16 (8 bytes) at a time, dq / dk / dv written as bf16 pairs (4 bytes), lse / delta are fp32
+  {
+    const char* bad = misaligned(a->o, 8) ? "o" : misaligned(a->d_o, 8) ? "d_o" : misaligned(a->dq, 4) ? "dq"
+                    : misaligned(a->dk, 4) ? "dk" : misaligned(a->dv, 4) ? "dv" : misaligned(a->lse, 4) ? "lse"
+                    : misaligned(a->delta, 4) ? "delta" : nullptr;
+    if (bad) return fail(DPIPE_EINVAL, "dpipe_attn_bwd: %s misaligned (o / d_o 8-byte, the others 4-byte alignment)", bad);
+  }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const int B = a->batch, H = a->heads, Lq = a->seq_q, Lk = a->seq_k;
-  {
-    const int64_t warps = (int64_t)B * Lq * H;
-    const int wpb = 8;
-    attn_bwd_delta_kernel<<<(unsigned)((warps + wpb - 1) / wpb), wpb * 32, 0, s>>>(
-        reinterpret_cast<const __nv_bfloat16*>(a->o), a->ldo, reinterpret_cast<const __nv_bfloat16*>(a->d_o), a->lddo,
-        a->delta, B, H, Lq);
-  }
   // 128-row boxes for the tile a CTA owns, 64-row boxes for the chunks it streams
   CUtensorMap tq, tk, tv, tdo, tq64, tk64, tv64, tdo64;
   const uint64_t bh = (uint64_t)B * H;
@@ -378,6 +378,14 @@ extern "C" int dpipe_attn_bwd(const dpipe_attn_bwd_args* a, void* stream) {
     const uint32_t box64[4] = {64, BC, 1, 1};
     if ((rc = make_tmap_4d_bf16(&tdo, a->d_o, dims, strides, box))) return rc;
     if ((rc = make_tmap_4d_bf16(&tdo64, a->d_o, dims, strides, box64))) return rc;
+  }
+  // every argument is checked and every tensor map encoded before the first launch
+  {
+    const int64_t warps = (int64_t)B * Lq * H;
+    const int wpb = 8;
+    attn_bwd_delta_kernel<<<(unsigned)((warps + wpb - 1) / wpb), wpb * 32, 0, s>>>(
+        reinterpret_cast<const __nv_bfloat16*>(a->o), a->ldo, reinterpret_cast<const __nv_bfloat16*>(a->d_o), a->lddo,
+        a->delta, B, H, Lq);
   }
   static bool configured = false;
   if (!configured) {

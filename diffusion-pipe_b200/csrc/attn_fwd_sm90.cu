@@ -215,6 +215,9 @@ extern "C" int dpipe_attn_fwd(const dpipe_attn_args* a, void* stream) {
   if (a->batch <= 0 || a->heads <= 0 || a->seq_q <= 0 || a->seq_k <= 0)
     return fail(DPIPE_EINVAL, "dpipe_attn_fwd: empty problem");
   if (a->ldo % 8 != 0 || a->ldo < (int64_t)a->heads * HD) return fail(DPIPE_EINVAL, "dpipe_attn_fwd: bad ldo");
+  // o is written as bf16 pairs (4 bytes), lse as fp32
+  if (misaligned(a->o, 4)) return fail(DPIPE_EINVAL, "dpipe_attn_fwd: o misaligned (needs 4-byte alignment)");
+  if (misaligned(a->lse, 4)) return fail(DPIPE_EINVAL, "dpipe_attn_fwd: lse misaligned (needs 4-byte alignment)");
   CUtensorMap tq, tk, tv;
   const uint64_t bh = (uint64_t)a->batch * a->heads;
   int rc;

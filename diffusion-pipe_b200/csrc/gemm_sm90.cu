@@ -461,6 +461,34 @@ extern "C" int dpipe_gemm_bf16(const dpipe_gemm_args* a, void* stream) {
       return fail(DPIPE_EINVAL, "dpipe_gemm_bf16: qkv stream does not fit the joint sequence");
     if (e.n_qkv < a->N && !a->out) return fail(DPIPE_EINVAL, "dpipe_gemm_bf16: fused linear1 needs an MLP output");
   }
+  // the epilogue moves 8 bf16 (16 bytes) per access through every pointer it uses except the fp32 rstd rows
+  {
+    const bool has_out2 = a->epilogue == DPIPE_EPI_BIAS_GELU || a->epilogue == DPIPE_EPI_GATE_RES ||
+                          a->epilogue == DPIPE_EPI_QKV_ROPE;
+    const bool has_aux = a->epilogue == DPIPE_EPI_GATE_RES || a->epilogue == DPIPE_EPI_MUL_GELU_GRAD;
+    const char* bad = nullptr;
+    if (misaligned(a->out, 16)) bad = "out";
+    else if (has_out2 && a->out2 && (misaligned(a->out2, 16) || a->ldo2 % 8 != 0)) bad = "out2/ldo2";
+    else if (a->bias && misaligned(a->bias, 16)) bad = "bias";
+    else if (has_aux && (misaligned(a->aux, 16) || a->ldaux % 8 != 0)) bad = "aux/ldaux";
+    else if (a->epilogue == DPIPE_EPI_GATE_RES && (misaligned(a->gate, 16) || a->gate_stride % 8 != 0)) bad = "gate/gate_stride";
+    if (!bad && a->epilogue == DPIPE_EPI_QKV_ROPE) {
+      const dpipe_qkv_epilogue& e = p.qkv;
+      if (misaligned(e.q, 16)) bad = "qkv.q";
+      else if (misaligned(e.k, 16)) bad = "qkv.k";
+      else if (misaligned(e.v, 16)) bad = "qkv.v";
+      else if (misaligned(e.qhat, 16)) bad = "qkv.qhat";
+      else if (misaligned(e.khat, 16)) bad = "qkv.khat";
+      else if (misaligned(e.q_norm_w, 16)) bad = "qkv.q_norm_w";
+      else if (misaligned(e.k_norm_w, 16)) bad = "qkv.k_norm_w";
+      else if (misaligned(e.rope_cos, 16)) bad = "qkv.rope_cos";
+      else if (misaligned(e.rope_sin, 16)) bad = "qkv.rope_sin";
+      else if (misaligned(e.q_rstd, 4)) bad = "qkv.q_rstd";
+      else if (misaligned(e.k_rstd, 4)) bad = "qkv.k_rstd";
+    }
+    if (bad) return fail(DPIPE_EINVAL, "dpipe_gemm_bf16: %s misaligned (pointers 16-byte aligned, fp32 rstd 4-byte, "
+                                       "leading dimensions multiples of 8 elements)", bad);
+  }
 
   CUtensorMap ta, tb;
   int rc;

@@ -35,4 +35,7 @@ int make_tmap_4d_bf16(CUtensorMap* out, const void* base, const uint64_t dims[4]
 
 int num_sms();  // SM count of the current device (cached per device)
 
+// true when `p` is not a multiple of `bytes`, the width of the vector loads / stores a kernel makes through it
+inline bool misaligned(const void* p, int bytes) { return (reinterpret_cast<uintptr_t>(p) & (uintptr_t)(bytes - 1)) != 0; }
+
 }  // namespace dpipe

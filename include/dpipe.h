@@ -85,6 +85,10 @@ typedef struct dpipe_gemm_args {
   const dpipe_qkv_epilogue* qkv; /* required for DPIPE_EPI_QKV_ROPE */
 } dpipe_gemm_args;
 
+/* Alignment (refused with DPIPE_EINVAL before any launch): A and B are TMA operands, 16-byte aligned with lda / ldb
+ * multiples of 8.  The epilogue accesses 16 bytes at a time, so out, bias and every out2 / aux / gate the epilogue uses
+ * are 16-byte aligned and ldo / ldo2 / ldaux / gate_stride multiples of 8; so are qkv->q, k, v, qhat, khat, q_norm_w,
+ * k_norm_w, rope_cos and rope_sin, while q_rstd / k_rstd need 4 bytes. */
 int dpipe_gemm_bf16(const dpipe_gemm_args* args, void* stream);
 
 /* ------------------------------------------------------------------------------------------ */
@@ -122,6 +126,10 @@ typedef struct dpipe_attn_bwd_args {
   float scale;
 } dpipe_attn_bwd_args;
 
+/* Alignment (refused with DPIPE_EINVAL before any launch): q, k, v and d_o are TMA operands, 16-byte aligned; ldo and
+ * lddo multiples of 8.  The forward writes o in 4-byte pairs and lse as fp32: both 4-byte aligned.  The backward reads
+ * o and d_o 8 bytes at a time (8-byte aligned) and writes dq / dk / dv in 4-byte pairs and lse / delta as fp32 (4-byte
+ * aligned). */
 /* backward of dpipe_attn_fwd; replaces flash-attn / SDPA backward reached via autograd from models/flux.py:502,525 */
 int dpipe_attn_bwd(const dpipe_attn_bwd_args* args, void* stream);
 

@@ -203,3 +203,95 @@ def test_struct_field_offsets_match_the_c_compiler(tmp_path):
         got = [getattr(cls, fn).offset for fn, _ in cls._fields_]
         assert got == want, (name, [fn for fn, _ in cls._fields_], fields[name], got, want)
         assert ctypes.sizeof(cls) == dict(c_off[name])['__size__'], name
+
+
+def _tmap_refused(lib):
+    """the tensor-map encode refused the call (without a driver it cannot even be looked up: refused all the same)"""
+    msg = lib.dpipe_last_error()
+    return b'TMA operand' in msg or b'cuTensorMapEncodeTiled entry point not available' in msg
+
+
+def _gemm_args(epilogue, qkv=None):
+    """a GEMM whose A is a TMA operand at address 8: whatever else is wrong, the tensor-map encode refuses the call, so a
+    field whose own alignment check were missing could still not reach a launch (every other pointer is aligned)"""
+    a = _lib.GemmArgs()
+    a.A, a.lda, a.B, a.ldb = 8, 64, 256, 64
+    a.M, a.N, a.K = 64, 768, 64
+    a.epilogue = epilogue
+    a.out, a.ldo, a.out2, a.ldo2 = 256, 768, 256, 768
+    a.aux, a.ldaux, a.gate, a.gate_stride = 256, 768, 256, 768
+    a.bias = 256
+    a.rows_per_batch, a.cta_group = 64, 1
+    if qkv is not None:
+        a.qkv = ctypes.pointer(qkv)
+    return a
+
+
+def _qkv_args():
+    e = _lib.QkvEpilogue()
+    for f in ('q', 'k', 'v', 'qhat', 'khat', 'q_norm_w', 'k_norm_w', 'rope_cos', 'rope_sin', 'q_rstd', 'k_rstd'):
+        setattr(e, f, 256)
+    e.heads, e.seq_total, e.seq_offset, e.n_qkv, e.eps = 2, 64, 0, 768, 1e-6
+    return e
+
+
+def test_gemm_refuses_misaligned_epilogue_pointers_before_any_launch():
+    """out, bias, out2 / ldo2, aux / ldaux, gate / gate_stride and the QKV pointers are read or written 16 bytes at a
+    time by the epilogue (q_rstd / k_rstd 4 bytes); none is a TMA operand, so the entry point checks them itself"""
+    lib = _lib.lib()
+    for epi in (_lib.EPI_STORE, _lib.EPI_BIAS_GELU, _lib.EPI_GATE_RES, _lib.EPI_MUL_GELU_GRAD, _lib.EPI_QKV_ROPE):
+        a = _gemm_args(epi, _qkv_args())
+        assert lib.dpipe_gemm_bf16(ctypes.byref(a), None) < 0 and _tmap_refused(lib), epi
+    cases = [(_lib.EPI_STORE, 'out', 264, b'out'), (_lib.EPI_STORE, 'bias', 258, b'bias'),
+             (_lib.EPI_BIAS_GELU, 'bias', 264, b'bias'), (_lib.EPI_BIAS_GELU, 'out2', 264, b'out2/ldo2'),
+             (_lib.EPI_BIAS_GELU, 'ldo2', 770, b'out2/ldo2'), (_lib.EPI_GATE_RES, 'out2', 260, b'out2/ldo2'),
+             (_lib.EPI_GATE_RES, 'aux', 264, b'aux/ldaux'), (_lib.EPI_GATE_RES, 'ldaux', 772, b'aux/ldaux'),
+             (_lib.EPI_GATE_RES, 'gate', 264, b'gate/gate_stride'), (_lib.EPI_GATE_RES, 'gate_stride', 769, b'gate/gate_stride'),
+             (_lib.EPI_MUL_GELU_GRAD, 'aux', 258, b'aux/ldaux'), (_lib.EPI_MUL_GELU_GRAD, 'ldaux', 770, b'aux/ldaux'),
+             (_lib.EPI_QKV_ROPE, 'out2', 264, b'out2/ldo2')]
+    for epi, field, value, name in cases:
+        a = _gemm_args(epi, _qkv_args())
+        setattr(a, field, value)
+        assert lib.dpipe_gemm_bf16(ctypes.byref(a), None) < 0, (epi, field)
+        assert name + b' misaligned' in lib.dpipe_last_error(), (epi, field, lib.dpipe_last_error())
+    for field, value in (('q', 264), ('k', 264), ('v', 264), ('qhat', 264), ('khat', 264), ('q_norm_w', 258),
+                         ('k_norm_w', 264), ('rope_cos', 260), ('rope_sin', 264), ('q_rstd', 258), ('k_rstd', 257)):
+        e = _qkv_args()
+        setattr(e, field, value)
+        a = _gemm_args(_lib.EPI_QKV_ROPE, e)
+        assert lib.dpipe_gemm_bf16(ctypes.byref(a), None) < 0, field
+        assert b'qkv.' + field.encode() + b' misaligned' in lib.dpipe_last_error(), (field, lib.dpipe_last_error())
+    # pointers an epilogue does not touch are not checked (here STORE's out2 / aux / gate, and NULL outputs)
+    a = _gemm_args(_lib.EPI_STORE)
+    a.out2, a.aux, a.gate, a.ldo2 = 258, 258, 258, 3
+    assert lib.dpipe_gemm_bf16(ctypes.byref(a), None) < 0 and _tmap_refused(lib)
+    e = _qkv_args()
+    e.q_rstd = e.k_rstd = e.qhat = e.khat = None
+    a = _gemm_args(_lib.EPI_QKV_ROPE, e)
+    assert lib.dpipe_gemm_bf16(ctypes.byref(a), None) < 0 and _tmap_refused(lib)
+
+
+def test_attention_refuses_misaligned_outputs_before_any_launch():
+    """attention forward writes o in 4-byte pairs and lse as fp32; the backward reads o / d_o 8 bytes at a time and
+    writes dq / dk / dv in pairs, lse / delta as fp32.  q sits at address 8, so the tensor-map encode of q refuses
+    every one of these calls even without the checks, and the backward encodes every map before its first launch"""
+    lib = _lib.lib()
+    a = _abi.AttnArgs()
+    a.q, a.k, a.v, a.o, a.lse = 8, 256, 256, 256, 256
+    a.ldo, a.batch, a.heads, a.seq_q, a.seq_k, a.scale = 128, 1, 1, 64, 64, 0.1
+    assert lib.dpipe_attn_fwd(ctypes.byref(a), None) < 0 and _tmap_refused(lib)
+    for field, value in (('o', 258), ('lse', 258)):
+        setattr(a, field, value)
+        assert lib.dpipe_attn_fwd(ctypes.byref(a), None) < 0, field
+        assert f'{field} misaligned'.encode() in lib.dpipe_last_error(), (field, lib.dpipe_last_error())
+        setattr(a, field, 256)
+    b = _abi.AttnBwdArgs()
+    for f in ('k', 'v', 'o', 'd_o', 'lse', 'delta', 'dq', 'dk', 'dv'):
+        setattr(b, f, 256)
+    b.q, b.ldo, b.lddo, b.batch, b.heads, b.seq_q, b.seq_k, b.scale = 8, 128, 128, 1, 1, 64, 64, 0.1
+    assert lib.dpipe_attn_bwd(ctypes.byref(b), None) < 0 and _tmap_refused(lib)
+    for field, value in (('o', 260), ('d_o', 260), ('dq', 258), ('dk', 258), ('dv', 258), ('lse', 258), ('delta', 257)):
+        setattr(b, field, value)
+        assert lib.dpipe_attn_bwd(ctypes.byref(b), None) < 0, field
+        assert f'{field} misaligned'.encode() in lib.dpipe_last_error(), (field, lib.dpipe_last_error())
+        setattr(b, field, 256)

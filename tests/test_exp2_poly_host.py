@@ -2,7 +2,9 @@
 with the coefficients READ FROM THE HEADER, against exp2 in float64: the error bound the header states (1.0e-4 relative,
 far below one bf16 ulp = 3.9e-3, which is all a softmax probability keeps), the exponent assembly for negative and positive
 integer parts, the round-to-nearest split at half-integers, and the clamp.  The kernels themselves are checked on the GPU
-(tests/test_kernels_gpu.py: attention forward / backward with DPIPE_ATTN_FWD_POLY = 0, 2, 4)."""
+by tests/test_gemm_attn_gpu.py: the attention forward element by element with the default MUFU exponential, and
+test_attention_forward_poly_exponential runs the same checks with DPIPE_ATTN_FWD_POLY = 2 and 4, with the error bound
+widened by the relative error this file checks."""
 import os
 import re
 
