@@ -84,7 +84,9 @@ K0, K1 = 0.7978845608028654, 0.044715
 
 
 def gelu(u, off=()):
-    """gelu_tanh of an E input: tanhf's 2 ulp and the rounding of inner are carried through 0.5 u (1 + t)"""
+    """gelu_tanh of an E input: tanhf's 2 ulp and the rounding of inner are carried through 0.5 u (1 + t).  An input
+    off by u.e moves the output by at most |gelu'(u)| u.e + K0 u.e^2 / 2 (Taylor: |gelu_tanh''| <= gelu_tanh''(0) = K0),
+    so a u that the kernel rounded to the other bf16 neighbour (u.e one ulp) is within the bound where gelu curves."""
     x = u.v
     inner = K0 * (x + K1 * x ** 3)
     t = torch.tanh(inner)
@@ -92,7 +94,7 @@ def gelu(u, off=()):
     ai = K0 * (x.abs() + K1 * x.abs() ** 3)
     fn = C * U * (4 * v.abs() + 0.5 * x.abs() * (2 + 4 * ai * (1 - t * t)))
     d = 0.5 * (1 + t) + 0.5 * x * (1 - t * t) * K0 * (1 + 3 * K1 * x * x)
-    return E(v, (fn if _on('gelu', off) else 0 * v) + d.abs() * u.e)
+    return E(v, (fn if _on('gelu', off) else 0 * v) + d.abs() * u.e + 0.5 * K0 * u.e * u.e)
 
 
 def gelu_grad(x, off=()):

@@ -135,6 +135,22 @@ def test_fused_epilogues_accept_their_own_outputs():
             assert R.accepts(_as_kernel(e), e), name
 
 
+def test_bias_gelu_accepts_either_neighbour_at_a_rounding_tie():
+    """u = bf16(acc + bias) at an exact tie may round to either neighbour, and the kernel's gelu of that neighbour must
+    pass: a bound that carries the one-ulp flip through gelu' alone misses gelu's curvature over that ulp (at u = 2.859
+    the kernel's value is 1.00008 bounds away).  Found in place on an H100: the BIAS_GELU GEMM of a Qwen-Image block
+    (M = 390, N = 2048, K = 512), element (370, 1293), got -0.0038300 want -0.0036374 bound 1.924e-4.  Every tie
+    between adjacent bf16 values in [2^-20, 8) of either sign."""
+    pos = torch.arange(0x3580, 0x4100, dtype=torch.int32).to(torch.int16).view(torch.bfloat16).double()   # 2^-20 .. 8
+    for vals in (pos, -pos):
+        lo, hi = vals[:-1], vals[1:]
+        acc = R.E(((lo + hi) / 2)[:, None], torch.full((lo.numel(), 1), 1e-30, dtype=torch.float64))
+        ref = G.gemm_bias_gelu_ref(acc)
+        for nb in (lo, hi):
+            R.check(torch.nn.functional.gelu(nb.float(), approximate='tanh')[:, None], ref['out'], 'gelu of a neighbour',
+                    bf16_out=False)
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # QKV epilogue
 # ---------------------------------------------------------------------------------------------------------------
