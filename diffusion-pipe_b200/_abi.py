@@ -131,6 +131,8 @@ SIGNATURES['dpipe_prodigy_scratch_doubles'] = (c_int, [c_void_p, c_int, ctypes.P
 SIGNATURES['dpipe_prodigy_stats'] = (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int64, c_void_p])
 SIGNATURES['dpipe_prodigy_apply'] = (c_int, [c_void_p, c_int, c_void_p, c_void_p])
 SIGNATURES['dpipe_adamw8bit_step'] = (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p])
+SIGNATURES['dpipe_came_scratch_doubles'] = (c_int, [c_void_p, c_int, ctypes.POINTER(c_int64)])
+SIGNATURES['dpipe_came_step'] = (c_int, [c_void_p, c_int, ctypes.c_double, c_void_p, c_int64, c_void_p])
 SIGNATURES['dpipe_noise_pack'] = (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int64, c_int, c_int,
                                           c_int, c_void_p])
 SIGNATURES['dpipe_exec_create'] = (c_int, [c_int, c_int, ctypes.c_double, ctypes.POINTER(c_void_p)])
@@ -179,3 +181,12 @@ class Adamw8bitTensor(ctypes.Structure):
     _fields_ = [('p', c_void_p), ('g', c_void_p), ('state1', c_void_p), ('state2', c_void_p), ('absmax1', c_void_p),
                 ('absmax2', c_void_p), ('numel', c_int64), ('step_size', c_float), ('beta1', c_float),
                 ('beta2', c_float), ('eps_c2', c_float), ('decay', c_float), ('dtype', c_int)]
+
+
+class CameTensor(ctypes.Structure):
+    _fields_ = [('p', c_void_p), ('g', c_void_p), ('m', c_void_p), ('row', c_void_p), ('col', c_void_p),
+                ('res_row', c_void_p), ('res_col', c_void_p), ('v', c_void_p), ('fac', c_void_p), ('sums', c_void_p),
+                ('numel', c_int64), ('L', c_int64), ('R', c_int64), ('C', c_int64), ('lr', ctypes.c_double),
+                ('weight_decay', ctypes.c_double), ('beta1', ctypes.c_double), ('beta2', ctypes.c_double),
+                ('beta3', ctypes.c_double), ('eps1', ctypes.c_double), ('eps2', ctypes.c_double), ('dtype', c_int),
+                ('factored', c_int), ('fixed_decay', c_int)]

@@ -775,6 +775,110 @@ def prodigy_apply(args, state):
         torch.autograd.graph.increment_version(p)
 
 
+class CameArgs:
+    """The packed per-tensor arguments of CAME steps (include/dpipe.h dpipe_came_tensor), their workspaces and fp64
+    scratch, built once by `came_pack` and reused while the parameters, their state and the group options other than
+    lr stay the same.  It holds no gradients: `came_step` writes each step's gradient pointers and learning rates into
+    the packed array with one tensor copy each.  fac[i] / sums[i] are tensor i's views of the fp32 / fp64 workspaces
+    (clip divisor and factors / the fp64 sums of the last step)."""
+
+    def __init__(self, arr, params, state, fac, sums, scratch, launches):
+        self.arr, self.n = arr, len(params)
+        self.params, self.state = params, state             # the state tensors the array points at, kept alive
+        self.fac, self.sums, self.scratch = fac, sums, scratch
+        self.launches = launches
+        cols = ctypes.sizeof(_abi.CameTensor) // 8
+        self._g = torch.frombuffer(arr, dtype=torch.int64).view(-1, cols)[:self.n, _abi.CameTensor.g.offset // 8]
+        self._lr = torch.frombuffer(arr, dtype=torch.float64).view(-1, cols)[:self.n, _abi.CameTensor.lr.offset // 8]
+
+    def set_step(self, grads, lrs):
+        """point the packed entries at this step's gradients (same shape, dtype, device and contiguity as the
+        parameters) and learning rates"""
+        if len(grads) != self.n or len(lrs) != self.n:
+            raise ValueError(f'came: {len(grads)} gradients and {len(lrs)} learning rates for {self.n} parameters')
+        for i, (p, g) in enumerate(zip(self.params, grads)):
+            if g is None or g.dtype != p.dtype or g.shape != p.shape or g.get_device() != p.get_device() \
+                    or not g.is_contiguous():
+                got = 'None' if g is None else f'{g.dtype} {tuple(g.shape)} on {g.device}'
+                raise TypeError(f'came: grad {i} must be a contiguous {p.dtype} tensor of shape {tuple(p.shape)} '
+                                f'on {p.device}, got {got}')
+        if self.n:
+            self._g.copy_(torch.tensor([g.data_ptr() for g in grads], dtype=torch.int64))
+            self._lr.copy_(torch.tensor([float(x) for x in lrs], dtype=torch.float64))
+
+
+def came_workspace_sizes(shape):
+    """(fp32, fp64) workspace elements of one tensor (include/dpipe.h dpipe_came_tensor fac / sums)"""
+    f, L, R, C = automagic_dims(shape)
+    return (1 + 2 * (L * R + L * C), 1 + 2 * (L * R + L * C + L)) if f else (1, 1)
+
+
+def came_pack(params, m, row, col, res_row, res_col, v, weight_decay, betas, eps1, eps2, fixed_decay):
+    """CameArgs for the parameters of every param group in group order: per parameter its state exp_avg (m), and
+    exp_avg_sq_row / _col, exp_avg_res_row / _col (ndim >= 2: row / col / res_row / res_col, None otherwise) or
+    exp_avg_sq (v, None for ndim >= 2), contiguous CUDA tensors of its dtype (bf16 or fp32), and its group's
+    weight_decay, betas (beta1, beta2, beta3), eps1, eps2, fixed_decay."""
+    n = len(params)
+    if any(len(x) != n for x in (m, row, col, res_row, res_col, v, weight_decay, betas, eps1, eps2, fixed_decay)):
+        raise ValueError('came_pack: the argument lists differ in length')
+    arr = (_abi.CameTensor * max(1, n))()
+    sizes = [came_workspace_sizes(p.shape) for p in params]
+    dev = params[0].device if params else 'cpu'
+    fac_flat = torch.empty(max(1, sum(s[0] for s in sizes)), dtype=torch.float32, device=dev)
+    sums_flat = torch.zeros(max(1, sum(s[1] for s in sizes)), dtype=torch.float64, device=dev)
+    fac = list(torch.split(fac_flat[:sum(s[0] for s in sizes)], [s[0] for s in sizes])) if n else []
+    sums = list(torch.split(sums_flat[:sum(s[1] for s in sizes)], [s[1] for s in sizes])) if n else []
+
+    def need(t, what, i, p, shape):
+        if t is None or not t.is_cuda or t.dtype != p.dtype or tuple(t.shape) != tuple(shape) or not t.is_contiguous():
+            got = 'None' if t is None else f'{t.dtype} {tuple(t.shape)} on {t.device}'
+            raise TypeError(f'came: {what} {i} must be a contiguous CUDA {p.dtype} tensor of shape {tuple(shape)}, '
+                            f'got {got}')
+        return t.data_ptr()
+    for i, p in enumerate(params):
+        if p.dtype not in _GRAD_DTYPES:
+            raise TypeError(f'came: tensor {i} is {p.dtype}; the kernels take bf16 or fp32 weights')
+        f, L, R, C = automagic_dims(p.shape)
+        a = arr[i]
+        a.p = need(p, 'param', i, p, p.shape)
+        a.g = a.p                   # a valid pointer until came_step writes the step's gradient
+        a.m = need(m[i], 'exp_avg', i, p, p.shape)
+        if f:
+            a.row = need(row[i], 'exp_avg_sq_row', i, p, p.shape[:-1])
+            a.col = need(col[i], 'exp_avg_sq_col', i, p, p.shape[:-2] + p.shape[-1:])
+            a.res_row = need(res_row[i], 'exp_avg_res_row', i, p, p.shape[:-1])
+            a.res_col = need(res_col[i], 'exp_avg_res_col', i, p, p.shape[:-2] + p.shape[-1:])
+        else:
+            a.v = need(v[i], 'exp_avg_sq', i, p, p.shape)
+        a.fac, a.sums = fac[i].data_ptr(), sums[i].data_ptr()
+        a.numel, a.L, a.R, a.C = p.numel(), L, R, C
+        a.weight_decay, (a.beta1, a.beta2, a.beta3) = weight_decay[i], betas[i]
+        a.eps1, a.eps2 = eps1[i], eps2[i]
+        a.dtype, a.factored, a.fixed_decay = _GRAD_DTYPES[p.dtype], int(f), int(bool(fixed_decay[i]))
+    need_d = ctypes.c_int64()
+    check(lib().dpipe_came_scratch_doubles(arr, n, ctypes.byref(need_d)), 'dpipe_came_scratch_doubles')
+    scratch = torch.empty(max(1, need_d.value), dtype=torch.float64, device=dev)
+    nonempty = [p.ndim >= 2 for p in params if p.numel()]
+    launches = sum(10 if any(nonempty[k:k + 64]) else 3 for k in range(0, len(nonempty), 64))
+    return CameArgs(arr, list(params), (list(m), list(row), list(col), list(res_row), list(res_col), list(v)), fac,
+                    sums, scratch, launches)
+
+
+def came_step(args, grads, lrs, clip_threshold):
+    """One CAME step (include/dpipe.h dpipe_came_step) over every tensor of `args` with this step's gradients and
+    per-parameter learning rates: the state and the weights in place, no host synchronisation; the weights' version
+    counters move."""
+    global LAUNCHES
+    args.set_step(grads, lrs)
+    _e = _prof_begin()
+    check(lib().dpipe_came_step(args.arr, args.n, float(clip_threshold), args.scratch.data_ptr(), args.scratch.numel(),
+                                _stream()), 'dpipe_came_step')
+    _prof_end(_e, 0.0, 'came_step')
+    LAUNCHES += args.launches
+    for p in args.params:           # as automagic_apply: caches keyed on the version see the new weights
+        torch.autograd.graph.increment_version(p)
+
+
 _A8_DTYPE = None
 
 

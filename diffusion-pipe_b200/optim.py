@@ -396,6 +396,105 @@ class Prodigy(torch.optim.Optimizer):
         self._packed = (None, None)
 
 
+_CAME_FACTORED = ('exp_avg_sq_row', 'exp_avg_sq_col', 'exp_avg_res_row', 'exp_avg_res_col')
+
+
+class CAME(torch.optim.Optimizer):
+    """pytorch_optimizer's CAME (`type = 'CAME'`, the reference's fallback `getattr(pytorch_optimizer, type)`,
+    train.py:698-700): Adafactor's factored second moment, plus a factored "confidence" moment of the residual
+    (u - m)^2 that scales the momentum update.  Each step is one call over the parameters of all groups
+    (`ops.came_step`; csrc/came.cu), at most 10 launches per 64 parameters, with no host synchronisation.
+
+    pytorch_optimizer's constructor surface and defaults; lr, betas, weight_decay, fixed_decay, eps1 and eps2 are read
+    per group, `group['lr']` on every step (LR schedulers work); clip_threshold applies to the whole optimizer.
+    ams_bound=True, maximize=True, weight_decouple=False (the text's L2 term is added to the gradient after the update
+    is computed) and gradient_release are refused.  Parameters without a gradient are skipped and their step count
+    does not advance.  State per parameter, pytorch_optimizer's keys, allocated in the parameter's dtype: `step` (host
+    int), `exp_avg`, and `exp_avg_sq_row` / `exp_avg_sq_col` / `exp_avg_res_row` / `exp_avg_res_col` (ndim >= 2) or
+    `exp_avg_sq`: about 2 B per bf16 parameter (adamw_optimi: 6 B).  The text's `RMS` entry (the weights' RMS, written
+    every step and never read) is not kept, and dropped when a state dict that has it is loaded.  Parameters are bf16 /
+    fp32 CUDA tensors (fp16 and fp8 are refused here, CPU tensors at the step)."""
+
+    def __init__(self, params, lr=2e-4, betas=(0.9, 0.999, 0.9999), weight_decay=0.0, weight_decouple=True,
+                 fixed_decay=False, clip_threshold=1.0, ams_bound=False, eps1=1e-30, eps2=1e-16, maximize=False,
+                 gradient_release=False):
+        for flag, what in ((ams_bound, 'ams_bound=True'), (maximize, 'maximize=True'),
+                           (not weight_decouple, 'weight_decouple=False (L2 weight decay)'),
+                           (gradient_release, 'gradient_release (the step runs once after the backward pass)')):
+            if flag:
+                raise NotImplementedError(f'came: {what} is not supported')
+        if not 0.0 <= lr:
+            raise ValueError(f'invalid learning rate {lr}')
+        if len(betas) != 3 or not all(0.0 <= b < 1.0 for b in betas):
+            raise ValueError(f'invalid betas {betas}')
+        if not 0.0 <= weight_decay:
+            raise ValueError(f'invalid weight_decay {weight_decay}')
+        if not (0.0 <= eps1 and 0.0 <= eps2):
+            raise ValueError(f'invalid eps1 / eps2 {eps1} / {eps2}')
+        if not clip_threshold > 0.0:
+            raise ValueError(f'invalid clip_threshold {clip_threshold}')
+        self.clip_threshold = clip_threshold
+        defaults = dict(lr=lr, betas=tuple(betas), weight_decay=weight_decay, weight_decouple=True,
+                        fixed_decay=fixed_decay, ams_bound=False, eps1=eps1, eps2=eps2)
+        super().__init__(params, defaults)
+        for group in self.param_groups:
+            for p in group['params']:
+                if p.dtype not in (torch.bfloat16, torch.float32):
+                    raise TypeError(f'came: parameters must be bf16 or fp32 tensors, got {p.dtype}')
+        self._packed = (None, None)
+
+    def _init_state(self, p):
+        state = self.state[p]
+        state['step'] = 0
+        state['exp_avg'] = torch.zeros_like(p, memory_format=torch.contiguous_format)
+        if p.ndim >= 2:
+            for k in ('exp_avg_sq', 'exp_avg_res'):
+                state[k + '_row'] = torch.zeros(p.shape[:-1], dtype=p.dtype, device=p.device)
+                state[k + '_col'] = torch.zeros(p.shape[:-2] + p.shape[-1:], dtype=p.dtype, device=p.device)
+        else:
+            state['exp_avg_sq'] = torch.zeros_like(p, memory_format=torch.contiguous_format)
+        return state
+
+    def _args(self, ps):
+        """ops.CameArgs for the (parameter, group) pairs ps, rebuilt only when that list, a parameter's storage or a
+        group option other than lr changes (gradients and learning rates are passed to each step, not packed)"""
+        key = tuple((id(p), p.data_ptr(), g['weight_decay'], g['betas'], g['eps1'], g['eps2'], g['fixed_decay'])
+                    for p, g in ps)
+        if self._packed[0] != key:
+            sts = [self.state[p] if self.state[p] else self._init_state(p) for p, _ in ps]
+            self._packed = (key, ops.came_pack(
+                [p for p, _ in ps], [s['exp_avg'] for s in sts],
+                *[[s.get(k) for s in sts] for k in _CAME_FACTORED], [s.get('exp_avg_sq') for s in sts],
+                [g['weight_decay'] for _, g in ps], [tuple(g['betas']) for _, g in ps], [g['eps1'] for _, g in ps],
+                [g['eps2'] for _, g in ps], [g['fixed_decay'] for _, g in ps]))
+        return self._packed[1]
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        ps = [(p, group) for group in self.param_groups for p in group['params'] if p.grad is not None]
+        args = self._args(ps)
+        ops.came_step(args, [p.grad for p, _ in ps], [g['lr'] for _, g in ps], self.clip_threshold)
+        for p, _ in ps:
+            self.state[p]['step'] += 1
+        return loss
+
+    def load_state_dict(self, state_dict):
+        """torch's load (state tensors cast to the parameter's dtype and device), made contiguous; `RMS` dropped"""
+        super().load_state_dict(state_dict)
+        for st in self.state.values():
+            st.pop('RMS', None)
+            for k, v in st.items():
+                if torch.is_tensor(v) and k != 'step':
+                    st[k] = v.contiguous()
+            if torch.is_tensor(st.get('step')):
+                st['step'] = int(st['step'])
+        self._packed = (None, None)
+
+
 def dynamic_map(signed):
     """bitsandbytes' create_dynamic_map(signed) (8 bits, 7 exponent bits): for each decade 10^(i-6), i = 0..6, the
     midpoints of linspace(0.1, 1, 2^i + 1) (signed, mirrored to negative values) or of linspace(0.1, 1, 2^(i+1) + 1)

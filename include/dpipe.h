@@ -414,6 +414,51 @@ typedef struct dpipe_adamw8bit_tensor {
  * Bit-identical to oracle/adamw8bit_ref.py adamw8bit_emulated.
  * replaces: bitsandbytes.optim.AdamW8bit.step (train.py:650-700). */
 int dpipe_adamw8bit_step(const dpipe_adamw8bit_tensor* t, int n, const float* qmap1, const float* qmap2, void* stream);
+/* One parameter of a CAME step (pytorch_optimizer.CAME, built for `type = 'CAME'`).  p, g and the state m = exp_avg:
+ * numel elements of dtype (0 = bf16, 1 = fp32), contiguous, at any element offset.  factored != 0 (ndim >= 2): shape
+ * [L = prod(shape[:-2]), R, C]; row / res_row = exp_avg_sq_row / exp_avg_res_row [L*R], col / res_col =
+ * exp_avg_sq_col / exp_avg_res_col [L*C], all of dtype; otherwise v = exp_avg_sq [numel] of dtype.  The group's
+ * hyper-parameters as the Python floats the reference passes (the kernels use their fp32 roundings).
+ * fac (fp32) and sums (fp64), per tensor, written by the step:
+ *   fac  = [clip divisor]  factored: then r_sq [L*R], c_sq [L*C], r_res [L*R], c_res [L*C]   (1 + 2 (L*R + L*C))
+ *   sums = [sum u^2]       factored: then for sq, then for res: row sums [L*R], column sums [L*C], sums over R of
+ *          the new row statistics [L]                                                          (1 + 2 (L*R + L*C + L)) */
+typedef struct dpipe_came_tensor {
+    void* p;
+    const void* g;
+    void* m;
+    void* row;
+    void* col;
+    void* res_row;
+    void* res_col;
+    void* v;
+    float* fac;
+    double* sums;
+    int64_t numel, L, R, C;
+    double lr, weight_decay, beta1, beta2, beta3, eps1, eps2;
+    int dtype;
+    int factored;
+    int fixed_decay;
+} dpipe_came_tensor;
+/* doubles of fp64 scratch dpipe_came_step needs for these tensors (row / column partials and per-CTA sums of u^2 of
+ * the largest chunk of 64) */
+int dpipe_came_scratch_doubles(const dpipe_came_tensor* t, int n, int64_t* out);
+/* One CAME step over n parameters, up to 64 non-empty ones per launch group (10 launches per group with a factored
+ * tensor, 3 without), no host synchronisation.  Per tensor, in fp32 ops rounded to the dtype after each op:
+ *   u0 = g*g + eps1;  factored: row = fma(mean_C(u0), 1 - beta2, row * beta2), col likewise over R,
+ *                     u = (rsqrt(row / mean_R(row)) * rsqrt(col)) * g;   else: v = fma(u0, 1 - beta2, v * beta2),
+ *                     u = rsqrt(v) * g
+ *   clip divisor = max(fp32(sqrt(sum u^2)) / fp32(sqrt(numel)) / clip_threshold, 1);  u /= clip divisor
+ *   m = fma(u, 1 - beta1, m * beta1);  res = (u - m)^2 + eps2
+ *   factored: res_row / res_col as row / col with beta3 over res, upd = (rsqrt(res_row / mean) * rsqrt(res_col)) * m;
+ *   else: upd = m
+ *   p = p * (1 - weight_decay * (fixed_decay ? 1 : lr));  p = p - upd * lr
+ * rsqrt(x) = 1 / sqrt(x), both correctly rounded.  Means are fp64 sums (fixed-order folds: bitwise repeatable, no
+ * float atomics) divided in fp64 and rounded to fp32.  Empty tensors are skipped.  Bit-identical to
+ * oracle/came_ref.py came_param_emulated fed with the sums written here.
+ * replaces: CAME.step (train.py:698-700). */
+int dpipe_came_step(const dpipe_came_tensor* t, int n, double clip_threshold, double* scratch, int64_t scratch_len,
+                    void* stream);
 /* flow-matching noising of one batch on the device, fp32, IEEE-rounded multiplies and adds (bit-identical to the host ops):
  *   xt = (1 - t[b]) * x1 + t[b] * x0,   target = x0 - x1      x1, x0: [bs, c, frames, h, w] contiguous; t: [bs]
  * pack != 0 (frames == 1): both outputs in diffusers' packed layout [bs, (h/2)(w/2), 4c] (2x2 patches, channel-major).

@@ -8,10 +8,11 @@ Same CLI flags and TOML keys as the reference for everything on the hot path (SU
 `gradient_clipping`, `partition_method` / `partition_split`, `[optimizer]` (type adamw = torch's fused AdamW, adamw_optimi =
 optimi's AdamW with Kahan-summed bf16 weights on the fused step kernel, automagic = the reference's Automagic on its
 fused step kernels, prodigy = pytorch_optimizer's Prodigy on its fused step kernels with d kept on the device,
-adamw8bit = bitsandbytes' AdamW8bit (blockwise 8-bit moments) on its fused step kernel, sgd;
+adamw8bit = bitsandbytes' AdamW8bit (blockwise 8-bit moments) on its fused step kernel, came = pytorch_optimizer's CAME on
+its fused step kernels, sgd;
 `betas`, `weight_decay`, `eps`, `lr`, `kahan_sum`, `decouple_lr`, `max_lr`; automagic: `min_lr`, `max_lr`, `lr_bump`,
 `clip_threshold`, `beta2`; prodigy: `beta3`, `d0`, `d_coef`, `growth_rate`, `fixed_decay`, `bias_correction`,
-`safeguard_warmup`; `train/prodigy_d` is logged with the loss; adamw8bit: `min_8bit_size`), `lr_scheduler`, `warmup_steps`, `epochs`, `max_steps`, `save_every_n_*`,
+`safeguard_warmup`; `train/prodigy_d` is logged with the loss; adamw8bit: `min_8bit_size`; came: `betas` (three), `eps1`, `eps2`, `clip_threshold`, `fixed_decay`), `lr_scheduler`, `warmup_steps`, `epochs`, `max_steps`, `save_every_n_*`,
 `checkpoint_every_n_minutes`, `--resume_from_checkpoint`, `--reset_dataloader`, `--reset_optimizer`.
 
 What is deliberately NOT here (out of the hot path, SURVEY.md section 8): VAE / text-encoder caching of a raw image
@@ -275,6 +276,9 @@ def make_optimizer_factory(config, model, global_batch_size=1):
         if typ == 'adamw8bit':                          # bitsandbytes.optim.AdamW8bit (train.py:650-700): fused step kernel
             from diffusion_pipe_b200 import optim
             return optim.AdamW8bit(groups, gradient_release=config['optimizer'].get('gradient_release', False), **oc)
+        if typ == 'came':                               # pytorch_optimizer.CAME (train.py:698-700): fused step kernels
+            from diffusion_pipe_b200 import optim
+            return optim.CAME(groups, gradient_release=config['optimizer'].get('gradient_release', False), **oc)
         if typ == 'sgd':
             return torch.optim.SGD(groups, **oc)
         raise NotImplementedError(f'optimizer type {typ} is not wired into this driver (third-party optimizers are out of '
