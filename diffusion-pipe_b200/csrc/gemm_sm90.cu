@@ -1,7 +1,8 @@
-// Warp-specialised bf16 GEMM for sm_90a, one 128x256 output tile per CTA:
+// Warp-specialised persistent bf16 GEMM for sm_90a, 128x256 output tiles:
 //   TMA (128B-swizzled tiles) -> shared memory ring -> wgmma (two consumer warpgroups, 64 rows x 256 columns
-//   each, fp32 accumulators in registers) -> fp32 tile staged in shared memory (over the drained ring) ->
-//   one thread per row and column half runs the fused epilogue.
+//   each, fp32 accumulators in registers) -> fp32 tile staged, one 64-column quarter at a time, in a buffer of each
+//   warpgroup's own -> coalesced fused epilogue.  One CTA per SM walks the tiles; the producer warp keeps loading the
+//   next tile's k-blocks into the ring while the consumers run the epilogue of the last one.
 //
 //   D[M,N] = Aop[M,K] * Bop[N,K]^T.  Each operand may be K-major (reduction dim contiguous) or
 //   MN-major (non-reduced dim contiguous), so forward (X*W^T), dgrad (dY*W) and wgrad (dY^T*X) all run
@@ -28,10 +29,13 @@ constexpr int B_TILE_BYTES = BN * BK * 2;  // 32 KiB
 constexpr int SUB_BYTES = 64 * 64 * 2;     // one 64(mn) x 64(k) MN-major sub-tile = 8 KiB
 constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
 constexpr int STAGES = 4;                  // 192 KiB of operand staging
-constexpr int STG_LD = BN + 4;             // fp32 staging row stride: rows read 16 B at a time land in distinct banks
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-constexpr int GEMM_THREADS = 288;  // warps 0-7: two consumer warpgroups; warp 8: TMA producer
-static_assert(BM * STG_LD * 4 <= STAGES * STAGE_BYTES, "the fp32 staging tile must fit in the operand ring");
+constexpr int EPI_SMEM_BYTES = 2 * (64 * 64 * 4 + 64 * 4);  // each warpgroup: a fp32 64x64 quarter + 64 rstd
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_SMEM_BYTES + 256 /*barriers*/ + 1024 /*align slack*/;
+constexpr int GEMM_THREADS = 384;  // warps 0-7: two consumer warpgroups; warpgroup 2: warp 8 is the TMA producer
+// the producer warpgroup gives its registers to the consumers: 128 x 40 + 256 x 232 <= 64 Ki
+constexpr int PRODUCER_REGS = 40;
+constexpr int CONSUMER_REGS = 232;
+static_assert(SMEM_BYTES <= 227 * 1024, "ring, epilogue buffers and barriers must fit one SM's shared memory");
 
 struct GemmParams {
   int M, N, K;
@@ -52,224 +56,293 @@ struct GemmParams {
 };
 
 // ---------------------------------------------------------------------------------------------
-// epilogue helpers: every thread owns one staged row and walks it 32 columns at a time
+// epilogue: each consumer warpgroup stages its 64 rows of the tile one 64-column quarter at a time in a buffer of its
+// own (not the operand ring, so the producer keeps loading the next tile meanwhile) and drains the quarter row by row:
+// a thread takes 8 consecutive columns of 4 rows, so 8 lanes cover one row's 64 columns and every global access of a
+// warp touches 4 contiguous 128-byte row segments.  Each output element sees the same fp32 operations as when one
+// thread walked a whole row.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void load_bf16x32(const __nv_bfloat16* p, bool ok, float* f) {
-  if (ok) {
-    const uint4* v = reinterpret_cast<const uint4*>(p);
+constexpr int EPI_COLS = 64;          // columns per staged quarter
+constexpr int EPI_ROWS = 4;           // rows per thread and quarter
+constexpr int STG_FLOATS = 64 * EPI_COLS;
+
+// staged fp32 quarter [64 rows][64 columns]: the 16-byte chunk c of row r lives at chunk c ^ (r & 7), so both the
+// fragment writes (8 rows x 32 B per instruction) and the drain reads (4 rows x 128 B) take the fewest wavefronts
+__device__ __forceinline__ int stg_idx(int r, int c) { return r * EPI_COLS + ((((c >> 2) ^ r) & 7) << 2) + ((c >> 2) & 8) * 4 + (c & 3); }
+
+template <int Q>
+__device__ __forceinline__ void stage_q(const float* acc, float* stg, int r0, int c0) {
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      uint4 q = v[j];
-      f[j * 8 + 0] = bf16_lo(q.x); f[j * 8 + 1] = bf16_hi(q.x);
-      f[j * 8 + 2] = bf16_lo(q.y); f[j * 8 + 3] = bf16_hi(q.y);
-      f[j * 8 + 4] = bf16_lo(q.z); f[j * 8 + 5] = bf16_hi(q.z);
-      f[j * 8 + 6] = bf16_lo(q.w); f[j * 8 + 7] = bf16_hi(q.w);
-    }
+  for (int j = 0; j < 8; ++j) {
+    const int a = 4 * (8 * Q + j), c = 8 * j + c0;
+    *reinterpret_cast<float2*>(stg + stg_idx(r0, c)) = make_float2(acc[a], acc[a + 1]);
+    *reinterpret_cast<float2*>(stg + stg_idx(r0 + 8, c)) = make_float2(acc[a + 2], acc[a + 3]);
+  }
+}
+// accumulator columns [64q, 64q + 64) of the warpgroup's fragment -> stg (a switch keeps every acc index constant)
+__device__ __forceinline__ void stage_quarter(const float* acc, float* stg, int q, int w4, int lane) {
+  const int r0 = w4 * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+  switch (q) {
+    case 0: stage_q<0>(acc, stg, r0, c0); break;
+    case 1: stage_q<1>(acc, stg, r0, c0); break;
+    case 2: stage_q<2>(acc, stg, r0, c0); break;
+    default: stage_q<3>(acc, stg, r0, c0); break;
+  }
+}
+
+__device__ __forceinline__ void ld_stg8(const float* stg, int r, int c, float* f) {
+  const float4 lo = *reinterpret_cast<const float4*>(stg + stg_idx(r, c));
+  const float4 hi = *reinterpret_cast<const float4*>(stg + stg_idx(r, c + 4));
+  f[0] = lo.x; f[1] = lo.y; f[2] = lo.z; f[3] = lo.w; f[4] = hi.x; f[5] = hi.y; f[6] = hi.z; f[7] = hi.w;
+}
+__device__ __forceinline__ uint4 ld_u4(const void* p) { return *reinterpret_cast<const uint4*>(p); }
+__device__ __forceinline__ void unpack_bf16x8(uint4 q, float* f) {
+  f[0] = bf16_lo(q.x); f[1] = bf16_hi(q.x); f[2] = bf16_lo(q.y); f[3] = bf16_hi(q.y);
+  f[4] = bf16_lo(q.z); f[5] = bf16_hi(q.z); f[6] = bf16_lo(q.w); f[7] = bf16_hi(q.w);
+}
+__device__ __forceinline__ void load_bf16x8(const __nv_bfloat16* p, bool ok, float* f) {
+  if (ok) {
+    unpack_bf16x8(ld_u4(p), f);
   } else {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) f[j] = 0.f;
+    for (int j = 0; j < 8; ++j) f[j] = 0.f;
   }
 }
-__device__ __forceinline__ void store_bf16x32(__nv_bfloat16* p, const float* f) {
-  uint4* v = reinterpret_cast<uint4*>(p);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    uint4 q;
-    q.x = pack_bf16(f[j * 8 + 0], f[j * 8 + 1]);
-    q.y = pack_bf16(f[j * 8 + 2], f[j * 8 + 3]);
-    q.z = pack_bf16(f[j * 8 + 4], f[j * 8 + 5]);
-    q.w = pack_bf16(f[j * 8 + 6], f[j * 8 + 7]);
-    v[j] = q;
-  }
-}
-__device__ __forceinline__ void load_f32x32(const float* p, float* f) {
-  const float4* v = reinterpret_cast<const float4*>(p);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    float4 q = v[j];
-    f[j * 4 + 0] = q.x; f[j * 4 + 1] = q.y; f[j * 4 + 2] = q.z; f[j * 4 + 3] = q.w;
-  }
+__device__ __forceinline__ void store_bf16x8(__nv_bfloat16* p, const float* f) {
+  uint4 q;
+  q.x = pack_bf16(f[0], f[1]); q.y = pack_bf16(f[2], f[3]); q.z = pack_bf16(f[4], f[5]); q.w = pack_bf16(f[6], f[7]);
+  *reinterpret_cast<uint4*>(p) = q;
 }
 
-// bias + GELU(tanh) for one 32-column chunk; `col` is the global column of f[0]
-__device__ __forceinline__ void epi_bias_gelu_chunk(const GemmParams& p, bool ok, int row, int col,
-                                                    int out_col, float* acc) {
-  float b[32];
-  load_bf16x32(p.bias ? p.bias + col : nullptr, p.bias != nullptr, b);
-  float u[32], h[32];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    u[j] = bf16_round(acc[j] + b[j]);
-    h[j] = gelu_tanh(u[j]);
-  }
-  if (ok) {
-    if (p.out2) store_bf16x32(p.out2 + (int64_t)row * p.ldo2 + out_col, u);
-    store_bf16x32(p.out + (int64_t)row * p.ldo + out_col, h);
-  }
-}
-
-__device__ __forceinline__ void ld_row32(const float* s, uint32_t* r) {
-  const float4* v = reinterpret_cast<const float4*>(s);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    float4 q = v[j];
-    r[j * 4 + 0] = __float_as_uint(q.x); r[j * 4 + 1] = __float_as_uint(q.y);
-    r[j * 4 + 2] = __float_as_uint(q.z); r[j * 4 + 3] = __float_as_uint(q.w);
-  }
-}
-
+// one staged quarter of a non-QKV tile (and of the MLP half of the fused linear1); `col` is the global column of the
+// thread's first element, rows row0 + rw + 4i
 template <int EPI>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, int row, int n0, const float* srow, int half) {
-  // `half` selects which 128 of the tile's 256 accumulator columns this thread drains; srow is its staged fp32 row
-  const bool row_ok = row < p.M;
-  const int batch = row_ok ? row / p.rows_per_batch : 0;
-
-  if constexpr (EPI == DPIPE_EPI_QKV_ROPE) {
-    if (n0 < p.qkv.n_qkv) {
-      // ---- q / k / v columns: this 256-wide tile holds two heads of one of q, k, v ----
-      const dpipe_qkv_epilogue& e = p.qkv;
-      const int hd = e.heads * 128;
-      const int which = n0 / hd;  // 0 q, 1 k, 2 v (tile never straddles: hd % 256 == 0)
-      const int tok = row_ok ? row - batch * p.rows_per_batch : 0;
-      const int pos = e.seq_offset + tok;
-#pragma unroll 1
-      for (int hh = half; hh <= half; ++hh) {
-        const int col_h = n0 + hh * 128;  // global column of this head's first element
-        if (col_h >= p.N) break;
-        const int head = (col_h - which * hd) >> 7;
-        const int64_t o = (((int64_t)batch * e.heads + head) * e.seq_total + pos) * 128;
-        if (which == 2) {
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {
-            uint32_t r[32];
-            ld_row32(srow + hh * 128 + c * 32, r);
-            float b[32], f[32];
-            load_bf16x32(p.bias ? p.bias + col_h + c * 32 : nullptr, p.bias != nullptr, b);
+__device__ __forceinline__ void drain_quarter(const GemmParams& p, const float* stg, int row0, int rw, int cl, int col) {
+  if (col >= p.N) return;  // N % 8 == 0: a thread's 8 columns are all in or all out
+  float b[8];
+  load_bf16x8(p.bias ? p.bias + col : nullptr, p.bias != nullptr, b);
+  // every global input of the 4 rows is requested before the first is used
+  uint4 in0[EPI_ROWS], in1[EPI_ROWS];
 #pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(r[j]) + b[j];
-            if (row_ok) store_bf16x32(reinterpret_cast<__nv_bfloat16*>(e.v) + o + c * 32, f);
-          }
-        } else {
-          // pass 1: sum of squares of the bf16-rounded projection (reference: RMSNorm on the bf16 Linear output)
-          float ss = 0.f;
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {
-            uint32_t r[32];
-            ld_row32(srow + hh * 128 + c * 32, r);
-            float b[32];
-            load_bf16x32(p.bias ? p.bias + col_h + c * 32 : nullptr, p.bias != nullptr, b);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              float v = bf16_round(__uint_as_float(r[j]) + b[j]);
-              ss += v * v;
-            }
-          }
-          const float rstd = rsqrtf(ss * (1.0f / 128.0f) + e.eps);
-          const __nv_bfloat16* w = reinterpret_cast<const __nv_bfloat16*>(which == 0 ? e.q_norm_w : e.k_norm_w);
-          __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(which == 0 ? e.q : e.k);
-          __nv_bfloat16* dst_hat = reinterpret_cast<__nv_bfloat16*>(which == 0 ? e.qhat : e.khat);
-          float* dst_rstd = which == 0 ? e.q_rstd : e.k_rstd;
-          if (row_ok && dst_rstd) dst_rstd[((int64_t)batch * e.heads + head) * e.seq_total + pos] = rstd;
-          // pass 2: normalise, scale, rotate, store
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {
-            uint32_t r[32];
-            ld_row32(srow + hh * 128 + c * 32, r);
-            float b[32], wv[32], xh[32], y[32];
-            load_bf16x32(p.bias ? p.bias + col_h + c * 32 : nullptr, p.bias != nullptr, b);
-            load_bf16x32(w + c * 32, true, wv);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              float v = bf16_round(__uint_as_float(r[j]) + b[j]);
-              xh[j] = bf16_round(v * rstd);
-              y[j] = bf16_round(xh[j] * wv[j]);
-            }
-            if (row_ok) {
-              if (dst_hat) store_bf16x32(dst_hat + o + c * 32, xh);
-              float cs[32], sn[32], ro[32];
-              load_f32x32(e.rope_cos + (int64_t)pos * 128 + c * 32, cs);
-              load_f32x32(e.rope_sin + (int64_t)pos * 128 + c * 32, sn);
-#pragma unroll
-              for (int j = 0; j < 32; j += 2) {
-                ro[j] = y[j] * cs[j] - y[j + 1] * sn[j];
-                ro[j + 1] = y[j + 1] * cs[j + 1] + y[j] * sn[j + 1];
-              }
-              store_bf16x32(dst + o + c * 32, ro);
-            }
-          }
-        }
+  for (int i = 0; i < EPI_ROWS; ++i) {
+    const int row = row0 + rw + 4 * i;
+    const bool ok = row < p.M;
+    in0[i] = in1[i] = make_uint4(0, 0, 0, 0);
+    if constexpr (EPI == DPIPE_EPI_STORE) {
+      if (ok && p.accumulate) in0[i] = ld_u4(p.out + (int64_t)row * p.ldo + col);
+    } else if constexpr (EPI == DPIPE_EPI_GATE_RES) {
+      if (ok) {
+        in0[i] = ld_u4(p.aux + (int64_t)row * p.ldaux + col);
+        in1[i] = ld_u4(p.gate + (int64_t)(row / p.rows_per_batch) * p.gate_stride + col);
       }
-      return;
+    } else if constexpr (EPI == DPIPE_EPI_MUL_GELU_GRAD) {
+      if (ok) in0[i] = ld_u4(p.aux + (int64_t)row * p.ldaux + col);
     }
   }
-
-#pragma unroll 1
-  for (int c = half * 4; c < half * 4 + 4; ++c) {
-    const int col = n0 + c * 32;
-    if (col >= p.N) break;  // warp-uniform
-    uint32_t r[32];
-    ld_row32(srow + c * 32, r);
-    float acc[32];
 #pragma unroll
-    for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(r[j]);
-    const bool ok = row_ok && (col + 32 <= p.N);
-    const bool tail = row_ok && !ok;  // partial chunk at the right edge (N % 32 != 0)
-
+  for (int i = 0; i < EPI_ROWS; ++i) {
+    const int rl = rw + 4 * i, row = row0 + rl;
+    if (row >= p.M) continue;
+    float acc[8];
+    ld_stg8(stg, rl, cl, acc);
     if constexpr (EPI == DPIPE_EPI_STORE) {
-      float b[32];
-      load_bf16x32(p.bias ? p.bias + col : nullptr, p.bias != nullptr && col + 32 <= p.N, b);
-      if (p.bias && col + 32 > p.N) {
-        for (int j = 0; j < 32 && col + j < p.N; ++j) b[j] = __bfloat162float(p.bias[col + j]);
-      }
       __nv_bfloat16* dst = p.out + (int64_t)row * p.ldo + col;
-      if (ok) {
+      float old[8];
+      unpack_bf16x8(in0[i], old);
+      if ((col & ~31) + 32 <= p.N) {
         if (p.accumulate) {
-          float old[32];
-          load_bf16x32(dst, true, old);
 #pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] += old[j];
+          for (int j = 0; j < 8; ++j) acc[j] += old[j];
         }
 #pragma unroll
-        for (int j = 0; j < 32; ++j) acc[j] += b[j];
-        store_bf16x32(dst, acc);
-      } else if (tail) {
-        for (int j = 0; j < 32 && col + j < p.N; ++j) {
+        for (int j = 0; j < 8; ++j) acc[j] += b[j];
+        store_bf16x8(dst, acc);
+      } else {
+        // the partial 32-column group at the right edge (N % 32 != 0) adds the bias before the old value
+        __nv_bfloat16 o[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
           float v = acc[j] + b[j];
-          if (p.accumulate) v += __bfloat162float(dst[j]);
-          dst[j] = __float2bfloat16_rn(v);
+          if (p.accumulate) v += old[j];
+          o[j] = __float2bfloat16_rn(v);
         }
+        *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(o);
       }
-    } else if constexpr (EPI == DPIPE_EPI_BIAS_GELU) {
-      epi_bias_gelu_chunk(p, ok, row, col, col, acc);
-    } else if constexpr (EPI == DPIPE_EPI_QKV_ROPE) {
-      // columns beyond n_qkv: the MLP half of the fused linear1 of a single-stream block
-      epi_bias_gelu_chunk(p, ok, row, col, col - p.qkv.n_qkv, acc);
-    } else if constexpr (EPI == DPIPE_EPI_GATE_RES) {
-      float b[32], g[32], res[32], y[32], o[32];
-      load_bf16x32(p.bias ? p.bias + col : nullptr, p.bias != nullptr, b);
-      load_bf16x32(p.gate + (int64_t)batch * p.gate_stride + col, ok, g);
-      load_bf16x32(p.aux + (int64_t)row * p.ldaux + col, ok, res);
+    } else if constexpr (EPI == DPIPE_EPI_BIAS_GELU || EPI == DPIPE_EPI_QKV_ROPE) {
+      // QKV_ROPE: columns past n_qkv are the MLP half of the fused linear1 of a single-stream block
+      const int out_col = EPI == DPIPE_EPI_QKV_ROPE ? col - p.qkv.n_qkv : col;
+      float u[8], h[8];
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
+      for (int j = 0; j < 8; ++j) {
+        u[j] = bf16_round(acc[j] + b[j]);
+        h[j] = gelu_tanh(u[j]);
+      }
+      if (p.out2) store_bf16x8(p.out2 + (int64_t)row * p.ldo2 + out_col, u);
+      store_bf16x8(p.out + (int64_t)row * p.ldo + out_col, h);
+    } else if constexpr (EPI == DPIPE_EPI_GATE_RES) {
+      float res[8], g[8], y[8], o[8];
+      unpack_bf16x8(in0[i], res);
+      unpack_bf16x8(in1[i], g);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
         y[j] = bf16_round(acc[j] + b[j]);
         o[j] = res[j] + bf16_round(g[j] * y[j]);
       }
-      if (ok) {
-        if (p.out2) store_bf16x32(p.out2 + (int64_t)row * p.ldo2 + col, y);
-        store_bf16x32(p.out + (int64_t)row * p.ldo + col, o);
-      }
+      if (p.out2) store_bf16x8(p.out2 + (int64_t)row * p.ldo2 + col, y);
+      store_bf16x8(p.out + (int64_t)row * p.ldo + col, o);
     } else if constexpr (EPI == DPIPE_EPI_MUL_GELU_GRAD) {
-      float u[32], o[32];
-      load_bf16x32(p.aux + (int64_t)row * p.ldaux + col, ok, u);
+      float u[8], o[8];
+      unpack_bf16x8(in0[i], u);
 #pragma unroll
-      for (int j = 0; j < 32; ++j) o[j] = acc[j] * gelu_tanh_grad(u[j]);
-      if (ok) store_bf16x32(p.out + (int64_t)row * p.ldo + col, o);
+      for (int j = 0; j < 8; ++j) o[j] = acc[j] * gelu_tanh_grad(u[j]);
+      store_bf16x8(p.out + (int64_t)row * p.ldo + col, o);
     }
   }
 }
 
+// q / k / v columns of the fused QKV projection: the 256-wide tile holds two heads of one of q, k, v
+// (the tile never straddles: heads * 128 % 256 == 0)
+__device__ __forceinline__ void qkv_tile(const GemmParams& p, const float* acc, float* stg, float* rstd_s, int row0,
+                                         int n0, int w4, int lane, int bar_id) {
+  const dpipe_qkv_epilogue& e = p.qkv;
+  const int hd = e.heads * 128;
+  const int which = n0 / hd;  // 0 q, 1 k, 2 v
+  const int t = w4 * 32 + lane;
+  const int rw = w4 * 16 + (lane >> 3), cl = (lane & 7) * 8;
+  const __nv_bfloat16* w = reinterpret_cast<const __nv_bfloat16*>(which == 0 ? e.q_norm_w : e.k_norm_w);
+  __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(which == 0 ? e.q : which == 1 ? e.k : e.v);
+  __nv_bfloat16* dst_hat = reinterpret_cast<__nv_bfloat16*>(which == 0 ? e.qhat : e.khat);
+  float* dst_rstd = which == 0 ? e.q_rstd : e.k_rstd;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int col_h = n0 + hh * 128;  // global column of this head's first element
+    const int head = (col_h - which * hd) >> 7;
+    if (which == 2) {
+#pragma unroll
+      for (int qq = 0; qq < 2; ++qq) {
+        named_bar_sync(bar_id, 128);
+        stage_quarter(acc, stg, 2 * hh + qq, w4, lane);
+        named_bar_sync(bar_id, 128);
+        const int c = qq * 64 + cl;  // column inside the head
+        float b[8];
+        load_bf16x8(p.bias ? p.bias + col_h + c : nullptr, p.bias != nullptr, b);
+#pragma unroll
+        for (int i = 0; i < EPI_ROWS; ++i) {
+          const int rl = rw + 4 * i, row = row0 + rl;
+          if (row >= p.M) continue;
+          const int batch = row / p.rows_per_batch;
+          const int pos = e.seq_offset + row - batch * p.rows_per_batch;
+          const int64_t o = (((int64_t)batch * e.heads + head) * e.seq_total + pos) * 128;
+          float f[8];
+          ld_stg8(stg, rl, cl, f);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) f[j] += b[j];
+          store_bf16x8(dst + o + c, f);
+        }
+      }
+      continue;
+    }
+    // pass 1: thread t < 64 sums the squares of row t's 128 bf16-rounded projections in column order
+    // (reference: RMSNorm on the bf16 Linear output)
+    float ss = 0.f;
+#pragma unroll
+    for (int qq = 0; qq < 2; ++qq) {
+      named_bar_sync(bar_id, 128);
+      stage_quarter(acc, stg, 2 * hh + qq, w4, lane);
+      named_bar_sync(bar_id, 128);
+      if (t < 64) {
+#pragma unroll 1
+        for (int c = 0; c < EPI_COLS; c += 8) {
+          float b[8], r[8];
+          load_bf16x8(p.bias ? p.bias + col_h + qq * 64 + c : nullptr, p.bias != nullptr, b);
+          ld_stg8(stg, t, c, r);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            float v = bf16_round(r[j] + b[j]);
+            ss += v * v;
+          }
+        }
+      }
+    }
+    if (t < 64) {
+      const float rstd = rsqrtf(ss * (1.0f / 128.0f) + e.eps);
+      rstd_s[t] = rstd;
+      const int row = row0 + t;
+      if (row < p.M && dst_rstd) {
+        const int batch = row / p.rows_per_batch;
+        const int pos = e.seq_offset + row - batch * p.rows_per_batch;
+        dst_rstd[((int64_t)batch * e.heads + head) * e.seq_total + pos] = rstd;
+      }
+    }
+    // pass 2: normalise, scale, rotate, store; the head's second quarter is still staged, the first is staged again
+#pragma unroll
+    for (int qq = 1; qq >= 0; --qq) {
+      named_bar_sync(bar_id, 128);
+      if (qq == 0) {
+        stage_quarter(acc, stg, 2 * hh, w4, lane);
+        named_bar_sync(bar_id, 128);
+      }
+      const int c = qq * 64 + cl;
+      float b[8], wv[8];
+      load_bf16x8(p.bias ? p.bias + col_h + c : nullptr, p.bias != nullptr, b);
+      load_bf16x8(w + c, true, wv);
+#pragma unroll
+      for (int i = 0; i < EPI_ROWS; ++i) {
+        const int rl = rw + 4 * i, row = row0 + rl;
+        if (row >= p.M) continue;
+        const int batch = row / p.rows_per_batch;
+        const int pos = e.seq_offset + row - batch * p.rows_per_batch;
+        const int64_t o = (((int64_t)batch * e.heads + head) * e.seq_total + pos) * 128;
+        // the rope rows are requested first (registers allow one row's worth next to the live accumulators)
+        const float4* pc = reinterpret_cast<const float4*>(e.rope_cos + (int64_t)pos * 128 + c);
+        const float4* ps = reinterpret_cast<const float4*>(e.rope_sin + (int64_t)pos * 128 + c);
+        const float4 c0 = pc[0], c1 = pc[1], s0 = ps[0], s1 = ps[1];
+        const float rstd = rstd_s[rl];
+        float r[8], xh[8], y[8], ro[8];
+        ld_stg8(stg, rl, cl, r);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          float v = bf16_round(r[j] + b[j]);
+          xh[j] = bf16_round(v * rstd);
+          y[j] = bf16_round(xh[j] * wv[j]);
+        }
+        if (dst_hat) store_bf16x8(dst_hat + o + c, xh);
+        const float cs[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+        const float sn[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+#pragma unroll
+        for (int j = 0; j < 8; j += 2) {
+          ro[j] = y[j] * cs[j] - y[j + 1] * sn[j];
+          ro[j + 1] = y[j + 1] * cs[j + 1] + y[j] * sn[j + 1];
+        }
+        store_bf16x8(dst + o + c, ro);
+      }
+    }
+  }
+}
+
+// the fused epilogue of one tile for one consumer warpgroup: rows [row0, row0 + 64), columns [n0, n0 + 256)
+template <int EPI>
+__device__ __forceinline__ void epilogue_wg(const GemmParams& p, const float* acc, float* stg, float* rstd_s, int row0,
+                                            int n0, int w4, int lane, int bar_id) {
+  if constexpr (EPI == DPIPE_EPI_QKV_ROPE) {
+    if (n0 < p.qkv.n_qkv) {
+      qkv_tile(p, acc, stg, rstd_s, row0, n0, w4, lane, bar_id);
+      return;
+    }
+  }
+  const int rw = w4 * 16 + (lane >> 3), cl = (lane & 7) * 8;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    if (n0 + q * EPI_COLS >= p.N) break;  // uniform over the warpgroup: every thread meets the same barriers
+    named_bar_sync(bar_id, 128);           // the previous quarter is drained
+    stage_quarter(acc, stg, q, w4, lane);
+    named_bar_sync(bar_id, 128);
+    drain_quarter<EPI>(p, stg, row0, rw, cl, n0 + q * EPI_COLS + cl);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
-// the kernel
+// the kernel: persistent, CTA b takes tiles b, b + gridDim.x, ... (M fastest)
 // ---------------------------------------------------------------------------------------------
 template <bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
@@ -277,14 +350,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
                  const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+  float* stg_all = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);  // [2 warpgroups][STG_FLOATS]
+  float* rstd_all = stg_all + 2 * STG_FLOATS;                               // [2 warpgroups][64]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(rstd_all + 2 * 64);
   uint64_t* full_bar = bars;             // [STAGES]
   uint64_t* empty_bar = bars + STAGES;   // [STAGES]
 
   const uint32_t warp = warp_id_uniform();
   const uint32_t lane = lane_id();
-  const int mt = blockIdx.x % p.num_m_tiles, nt = blockIdx.x / p.num_m_tiles;
-  const int m0 = mt * BM, n0 = nt * BN;
   const int num_kb = (p.K + BK - 1) / BK;
 
   if (warp == 8 && elect_one()) {
@@ -298,84 +371,85 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constan
   }
   __syncthreads();
 
-  if (warp == 8) {
-    // ================= TMA producer =================
+  // `it` counts k-blocks over all of this CTA's tiles: ring stage it % STAGES, barrier phase (it / STAGES) & 1
+  if (warp >= 8) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp > 8) return;
+    // ================= TMA producer: runs ahead into the next tile's k-blocks as stages free up =================
     if (elect_one()) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int stage = kb % STAGES;
-        mbar_wait(smem_u32(&empty_bar[stage]), ((kb / STAGES) & 1) ^ 1);
-        const uint32_t a_dst = smem_u32(smem + stage * STAGE_BYTES);
-        const uint32_t b_dst = a_dst + A_TILE_BYTES;
-        const int k0 = kb * BK;
-        const uint32_t bar = smem_u32(&full_bar[stage]);
-        mbar_expect_tx(bar, STAGE_BYTES);
-        if constexpr (!A_MN) {
-          tma_load_2d(&tma_a, bar, a_dst, k0, m0);
-        } else {
-          tma_load_2d(&tma_a, bar, a_dst, m0, k0);
-          tma_load_2d(&tma_a, bar, a_dst + SUB_BYTES, m0 + 64, k0);
-        }
-        if constexpr (!B_MN) {
-          tma_load_2d(&tma_b, bar, b_dst, k0, n0, kEvictLast);
-        } else {
+      int it = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        const int m0 = (tile % p.num_m_tiles) * BM, n0 = (tile / p.num_m_tiles) * BN;
+        for (int kb = 0; kb < num_kb; ++kb, ++it) {
+          const int stage = it % STAGES;
+          mbar_wait(smem_u32(&empty_bar[stage]), ((it / STAGES) & 1) ^ 1);
+          const uint32_t a_dst = smem_u32(smem + stage * STAGE_BYTES);
+          const uint32_t b_dst = a_dst + A_TILE_BYTES;
+          const int k0 = kb * BK;
+          const uint32_t bar = smem_u32(&full_bar[stage]);
+          mbar_expect_tx(bar, STAGE_BYTES);
+          if constexpr (!A_MN) {
+            tma_load_2d(&tma_a, bar, a_dst, k0, m0);
+          } else {
+            tma_load_2d(&tma_a, bar, a_dst, m0, k0);
+            tma_load_2d(&tma_a, bar, a_dst + SUB_BYTES, m0 + 64, k0);
+          }
+          if constexpr (!B_MN) {
+            tma_load_2d(&tma_b, bar, b_dst, k0, n0, kEvictLast);
+          } else {
 #pragma unroll
-          for (int j = 0; j < BN / 64; ++j) tma_load_2d(&tma_b, bar, b_dst + j * SUB_BYTES, n0 + 64 * j, k0, kEvictLast);
+            for (int j = 0; j < BN / 64; ++j) tma_load_2d(&tma_b, bar, b_dst + j * SUB_BYTES, n0 + 64 * j, k0, kEvictLast);
+          }
         }
       }
     }
     return;
   }
 
-  // ================= consumer warpgroups: rows [64 wg, 64 wg + 64) of the tile =================
-  const int wg = warp >> 2;
-  float acc[128];
+  // ================= consumer warpgroups: rows [64 wg, 64 wg + 64) of each tile =================
+  setmaxnreg_inc<CONSUMER_REGS>();
+  const int wg = warp >> 2, w4 = warp & 3;
+  float* stg = stg_all + wg * STG_FLOATS;
+  float* rstd_s = rstd_all + wg * 64;
+  const int bar_id = 2 + wg;  // named barrier of this warpgroup's epilogue buffer (0 is __syncthreads)
+  int it = 0;
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const int m0 = (tile % p.num_m_tiles) * BM, n0 = (tile / p.num_m_tiles) * BN;
+    float acc[128];
 #pragma unroll
-  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-  for (int kb = 0; kb < num_kb; ++kb) {
-    const int stage = kb % STAGES;
-    mbar_wait(smem_u32(&full_bar[stage]), (kb / STAGES) & 1);
-    const uint32_t a_base = smem_u32(smem + stage * STAGE_BYTES);
-    const uint32_t b_base = a_base + A_TILE_BYTES;
-    wgmma_fence();
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      const int stage = (it + kb) % STAGES;
+      mbar_wait(smem_u32(&full_bar[stage]), ((it + kb) / STAGES) & 1);
+      const uint32_t a_base = smem_u32(smem + stage * STAGE_BYTES);
+      const uint32_t b_base = a_base + A_TILE_BYTES;
+      wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < BK / UK; ++k) {
-      // K-major: rows of this warpgroup start 64 rows (8 KiB) in; step 16 elements (32 B) inside the swizzle row.
-      // MN-major: sub-tile `wg` holds this warpgroup's 64 rows; step 16 k-rows = two 1024 B swizzle atoms.
-      const uint64_t adesc = A_MN ? make_smem_desc(a_base + wg * SUB_BYTES + k * 2048, SUB_BYTES, 1024)
-                                  : make_smem_desc(a_base + wg * (64 * 128) + k * 32, 16, 1024);
-      const uint64_t bdesc = B_MN ? make_smem_desc(b_base + k * 2048, SUB_BYTES, 1024)
-                                  : make_smem_desc(b_base + k * 32, 16, 1024);
-      wgmma_m64n256k16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, 1u);
+      for (int k = 0; k < BK / UK; ++k) {
+        // K-major: rows of this warpgroup start 64 rows (8 KiB) in; step 16 elements (32 B) inside the swizzle row.
+        // MN-major: sub-tile `wg` holds this warpgroup's 64 rows; step 16 k-rows = two 1024 B swizzle atoms.
+        const uint64_t adesc = A_MN ? make_smem_desc(a_base + wg * SUB_BYTES + k * 2048, SUB_BYTES, 1024)
+                                    : make_smem_desc(a_base + wg * (64 * 128) + k * 32, 16, 1024);
+        const uint64_t bdesc = B_MN ? make_smem_desc(b_base + k * 2048, SUB_BYTES, 1024)
+                                    : make_smem_desc(b_base + k * 32, 16, 1024);
+        wgmma_m64n256k16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, 1u);
+      }
+      wgmma_commit();
+      // keep one k-block of wgmma in flight; the previous one has retired, so its stage can be refilled
+      wgmma_wait<1>();
+      reg_fence<128>(acc);
+      if (kb > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(&empty_bar[(it + kb - 1) % STAGES]));
+      }
     }
-    wgmma_commit();
-    // keep one k-block of wgmma in flight; the previous one has retired, so its stage can be refilled
-    wgmma_wait<1>();
+    wgmma_wait<0>();
     reg_fence<128>(acc);
-    if (kb > 0) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&empty_bar[(kb - 1) % STAGES]));
-    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(&empty_bar[(it + num_kb - 1) % STAGES]));
+    it += num_kb;
+    epilogue_wg<EPI>(p, acc, stg, rstd_s, m0 + wg * 64, n0, w4, lane, bar_id);
   }
-  wgmma_wait<0>();
-  reg_fence<128>(acc);
-
-  // every TMA write has landed (all full barriers were waited on) and both warpgroups have retired their wgmma:
-  // the ring is free and holds the fp32 tile from here on
-  named_bar_sync(1, 256);
-  float* stg = reinterpret_cast<float*>(smem);
-  {
-    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    const int c0 = 2 * (lane & 3);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      *reinterpret_cast<float2*>(stg + r0 * STG_LD + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
-      *reinterpret_cast<float2*>(stg + (r0 + 8) * STG_LD + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-    }
-  }
-  named_bar_sync(1, 256);
-  const int r = threadIdx.x & (BM - 1);
-  const int half = threadIdx.x >> 7;
-  epilogue_tile<EPI>(p, m0 + r, n0, stg + r * STG_LD, half);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -389,7 +463,8 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams
     DPIPE_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     configured = true;
   }
-  kern<<<p.num_tiles, GEMM_THREADS, SMEM_BYTES, stream>>>(ta, tb, p);
+  const int grid = p.num_tiles < num_sms() ? p.num_tiles : num_sms();
+  kern<<<grid, GEMM_THREADS, SMEM_BYTES, stream>>>(ta, tb, p);
   DPIPE_CUDA_CHECK(cudaGetLastError());
   return 0;
 }

@@ -263,6 +263,12 @@ __device__ __forceinline__ f32x2 f2_exp2_mufu(f32x2 x) {
   return f2_pack(fast_exp2(x0), fast_exp2(x1));
 }
 
+// hand registers between warpgroups (every warp of the warpgroup executes the same call)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
