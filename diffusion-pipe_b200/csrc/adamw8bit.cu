@@ -15,6 +15,7 @@
 #include <cuda_bf16.h>
 
 #include "host_util.h"
+#include "optim_common.cuh"
 
 namespace dpipe {
 namespace {
@@ -30,10 +31,6 @@ struct A8List {
   long long blk0[A8_MAX + 1];             // prefix sums of the 256-element blocks per tensor
   int n;
 };
-
-__device__ __forceinline__ float round_to(bool bf16, float x) {
-  return bf16 ? __bfloat162float(__float2bfloat16_rn(x)) : x;
-}
 
 // number of midpoints below x: the nearest map entry (tree[1..255] in breadth-first order; NaN goes left: 0)
 __device__ __forceinline__ int nearest_code(const float* __restrict__ tree, float x) {
@@ -163,8 +160,8 @@ __device__ __forceinline__ void a8_lane(const dpipe_adamw8bit_tensor& t, long lo
   for (int j = 0; j < A8_PER_LANE; ++j) {
     if (Q8 && !isfinite(g[j])) continue;                                 // bnb skips the element: p stays
     const float den = __fadd_rn(__fsqrt_rn(v[j]), t.eps_c2);
-    const float pn = round_to(BF16, __fadd_rn(p[j], __fmul_rn(t.step_size, __fdiv_rn(m[j], den))));
-    p[j] = round_to(BF16, __fmul_rn(pn, t.decay));
+    const float pn = R<BF16>(__fadd_rn(p[j], __fmul_rn(t.step_size, __fdiv_rn(m[j], den))));
+    p[j] = R<BF16>(__fmul_rn(pn, t.decay));
   }
   store8<BF16>(t.p, e, valid, vec, p);
   if (!Q8) return;

@@ -21,13 +21,13 @@
 #include <cuda_bf16.h>
 
 #include "host_util.h"
+#include "optim_common.cuh"
 
 namespace dpipe {
 namespace {
 
 constexpr int AM_MAX = 64;
 constexpr int AM_THREADS = 256;
-constexpr int AM_TILE = 128;            // reduce tile: 128 rows (16 per warp) x 128 columns (4 per lane)
 constexpr int AM_WS_HEAD = 4;           // ws[0] clip divisor, ws[1] lr absmax, ws[2] avg_lr, ws[3] fp32(previous scale)
 
 struct AmList {
@@ -44,38 +44,6 @@ struct AmScal {
   float beta2, alpha, eps, bump, min_lr, max_lr, clip, neg_wd;
   int has_wd;
 };
-
-__device__ __forceinline__ float rnd(float x, bool r) { return r ? __bfloat162float(__float2bfloat16_rn(x)) : x; }
-__device__ __forceinline__ float bf(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
-__device__ __forceinline__ float rsqrt_rn(float x) { return __fdiv_rn(1.0f, __fsqrt_rn(x)); }   // torch: 1 / sqrt(x)
-
-__device__ __forceinline__ float ld(const void* a, long long j, int dt) {
-  return dt == 0 ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(a)[j]) : reinterpret_cast<const float*>(a)[j];
-}
-
-__device__ __forceinline__ int find(const long long* pre, int n, long long b) {
-  int i = 0;
-  while (i + 1 < n && b >= pre[i + 1]) ++i;
-  return i;
-}
-
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-  return v;
-}
-
-// deterministic block sum (fixed tree); the result is valid in every thread
-__device__ __forceinline__ double block_sum(double v, double* red) {
-  v = warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < AM_THREADS / 32; ++w) s += red[w];
-  return s;
-}
 
 __device__ __forceinline__ float new_lr(float u, signed char code, unsigned char pol, float scale, const AmScal& s) {
   const float mask = __fmul_rn((float)code, scale);                          // lr_mask = q.float() * scale
@@ -99,51 +67,26 @@ struct RowCol {
   }
 };
 
+// u0 = grad**2 + eps of a tile element, in fp32 at every step
+struct U0 {
+  const dpipe_automagic_tensor& T;
+  float eps;
+  __device__ __forceinline__ float row(long long, long long) const { return 0.f; }
+  __device__ __forceinline__ float col(long long, long long) const { return 0.f; }
+  __device__ __forceinline__ float operator()(long long j, float, float) const {
+    const float g = ld_dt(T.g, j, T.dtype);
+    return __fadd_rn(__fmul_rn(g, g), eps);
+  }
+};
+
 __global__ void __launch_bounds__(AM_THREADS) am_reduce_kernel(const __grid_constant__ AmList tl, const AmScal s,
                                                               double* __restrict__ scratch) {
-  __shared__ double colred[AM_THREADS / 32][AM_TILE];
+  __shared__ double colred[AM_THREADS / 32 * FM_TILE];
   long long b = blockIdx.x;
   const int i = find(tl.tiles0, tl.n, b);
   const dpipe_automagic_tensor& T = tl.t[i];
   b -= tl.tiles0[i];
-  const long long R = T.R, C = T.C, LR = T.L * R, LC = T.L * C;
-  const long long nstrip = (C + AM_TILE - 1) / AM_TILE, nrb = (R + AM_TILE - 1) / AM_TILE;
-  const long long strip = b % nstrip;
-  b /= nstrip;
-  const long long rb = b % nrb, l = b / nrb;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  double cacc[4] = {0.0, 0.0, 0.0, 0.0};
-  const long long c0 = strip * AM_TILE + lane;
-  for (int k = 0; k < AM_TILE / 8; ++k) {
-    const long long r = rb * AM_TILE + warp + 8 * k;
-    if (r >= R) break;                                                       // warp-uniform
-    const long long base = (l * R + r) * C;
-    float x[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) x[j] = c0 + 32 * j < C ? ld(T.g, base + c0 + 32 * j, T.dtype) : 0.f;
-    double rs = 0.0;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      if (c0 + 32 * j < C) {
-        const double u0 = __fadd_rn(__fmul_rn(x[j], x[j]), s.eps);         // grad**2 + eps
-        rs += u0;
-        cacc[j] += u0;
-      }
-    }
-    rs = warp_sum(rs);
-    if (lane == 0) scratch[tl.rp[i] + strip * LR + l * R + r] = rs;
-  }
-#pragma unroll
-  for (int j = 0; j < 4; ++j) colred[warp][lane + 32 * j] = cacc[j];
-  __syncthreads();
-  if (threadIdx.x < AM_TILE) {
-    const long long c = strip * AM_TILE + threadIdx.x;
-    if (c < C) {
-      double a = 0.0;
-      for (int w = 0; w < AM_THREADS / 32; ++w) a += colred[w][threadIdx.x];
-      scratch[tl.cp[i] + rb * LC + l * C + c] = a;
-    }
-  }
+  fm_tile<AM_THREADS>(FmGeom{T.L, T.R, T.C}, b, scratch, tl.rp[i], tl.cp[i], colred, U0{T, s.eps});
 }
 
 // one thread per row (then per column) of a factored tensor: fold the partials, EMA, column factors
@@ -155,11 +98,12 @@ __global__ void __launch_bounds__(AM_THREADS) am_fold_kernel(const __grid_consta
   b -= tl.fold0[i];
   const bool r = T.flags & DPIPE_AUTOMAGIC_ROUND_BF16;
   const long long R = T.R, C = T.C, LR = T.L * R, LC = T.L * C;
-  const long long nrowcta = (LR + AM_THREADS - 1) / AM_THREADS;
+  const FmGeom f{T.L, R, C};
+  const long long nrowcta = f.row_ctas(AM_THREADS);
   if (b < nrowcta) {
     const long long q = b * AM_THREADS + threadIdx.x;
     if (q >= LR) return;
-    const long long nstrip = (C + AM_TILE - 1) / AM_TILE;
+    const long long nstrip = f.nstrip();
     double a = 0.0;
     for (long long st = 0; st < nstrip; ++st) a += scratch[tl.rp[i] + st * LR + q];
     const float mean = __double2float_rn(a / (double)C);                     // update.mean(dim=-1)
@@ -168,7 +112,7 @@ __global__ void __launch_bounds__(AM_THREADS) am_fold_kernel(const __grid_consta
   } else {
     const long long q = (b - nrowcta) * AM_THREADS + threadIdx.x;
     if (q >= LC) return;
-    const long long nrb = (R + AM_TILE - 1) / AM_TILE;
+    const long long nrb = f.nrb();
     double a = 0.0;
     for (long long k = 0; k < nrb; ++k) a += scratch[tl.cp[i] + k * LC + q];
     const float mean = __double2float_rn(a / (double)R);                     // update.mean(dim=-2)
@@ -190,7 +134,7 @@ __global__ void __launch_bounds__(AM_THREADS) am_rowmean_kernel(const __grid_con
   const float* row = T.row + l * R;
   double a = 0.0;
   for (long long k = threadIdx.x; k < R; k += AM_THREADS) a += row[k];
-  a = block_sum(a, red);
+  a = block_sum<AM_THREADS>(a, red);
   const float rm = rnd(__double2float_rn(a / (double)R), r);
   if (threadIdx.x == 0) T.ws[AM_WS_HEAD + l] = rm;
   float* rf = T.ws + AM_WS_HEAD + T.L + l * R;
@@ -217,7 +161,7 @@ __global__ void __launch_bounds__(AM_THREADS) am_lr_kernel(const __grid_constant
       RowCol rc(tid, nthreads, C);
       for (long long j = tid; j < T.numel; j += nthreads, rc.next(C)) {
         const long long l = T.L == 1 ? 0 : rc.q / T.R;
-        const float u = u_factored(rf[rc.q], cf[l * C + rc.c], ld(T.g, j, T.dtype), r);
+        const float u = u_factored(rf[rc.q], cf[l * C + rc.c], ld_dt(T.g, j, T.dtype), r);
         sumsq += (double)u * (double)u;
         const float nl = new_lr(u, T.code[j], T.pol[j], scale, s);
         lrsum += nl;
@@ -225,7 +169,7 @@ __global__ void __launch_bounds__(AM_THREADS) am_lr_kernel(const __grid_constant
       }
     } else {
       for (long long j = tid; j < T.numel; j += nthreads) {
-        const float g = ld(T.g, j, T.dtype);
+        const float g = ld_dt(T.g, j, T.dtype);
         const float v = rnd(__fmaf_rn(__fadd_rn(__fmul_rn(g, g), s.eps), s.alpha, rnd(__fmul_rn(T.v[j], s.beta2), r)), r);
         T.v[j] = v;
         const float u = rnd(__fmul_rn(rnd(rsqrt_rn(v), r), g), r);           // exp_avg_sq.rsqrt().mul_(grad)
@@ -235,8 +179,8 @@ __global__ void __launch_bounds__(AM_THREADS) am_lr_kernel(const __grid_constant
         amax = fmaxf(amax, fabsf(nl));
       }
     }
-    sumsq = block_sum(sumsq, red);
-    lrsum = block_sum(lrsum, red);
+    sumsq = block_sum<AM_THREADS>(sumsq, red);
+    lrsum = block_sum<AM_THREADS>(lrsum, red);
     float w = amax;
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) w = fmaxf(w, __shfl_xor_sync(0xffffffffu, w, off));
@@ -270,8 +214,8 @@ __global__ void __launch_bounds__(AM_THREADS) am_finish_kernel(const __grid_cons
     lrsum += part[3 * k + 1];
     amax = fmaxf(amax, (float)part[3 * k + 2]);
   }
-  sumsq = block_sum(sumsq, red);
-  lrsum = block_sum(lrsum, red);
+  sumsq = block_sum<AM_THREADS>(sumsq, red);
+  lrsum = block_sum<AM_THREADS>(lrsum, red);
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, off));
   if ((threadIdx.x & 31) == 0) mx[threadIdx.x >> 5] = amax;
@@ -304,7 +248,7 @@ __global__ void __launch_bounds__(AM_THREADS) am_apply_kernel(const __grid_const
     const long long C = fact ? T.C : 1;
     RowCol rc(tid, nthreads, C);
     for (long long j = tid; j < T.numel; j += nthreads, rc.next(C)) {
-      const float g = ld(T.g, j, T.dtype);
+      const float g = ld_dt(T.g, j, T.dtype);
       float u;
       if (fact) {
         const long long l = T.L == 1 ? 0 : rc.q / T.R;
@@ -319,13 +263,13 @@ __global__ void __launch_bounds__(AM_THREADS) am_apply_kernel(const __grid_const
       T.code[j] = (signed char)(int)qv;
       u = rnd(__fmul_rn(u, nl), r);                                            // update.mul_(new_lr)
       if (T.dtype == 0) {
-        const float p = ld(T.p, j, 0);
+        const float p = ld_dt(T.p, j, 0);
         float upd = -u;
         if (s.has_wd) upd = rnd(__fadd_rn(upd, __fmul_rn(__fmul_rn(p, s.neg_wd), nl)), r);
         __nv_bfloat16* sh = reinterpret_cast<__nv_bfloat16*>(T.shift) + j;
-        float shift = bf(__fadd_rn(__bfloat162float(*sh), upd));               // shift.add_(update)
-        const float pn = bf(__fadd_rn(p, shift));                              // p.add_(shift)
-        shift = bf(__fadd_rn(shift, __fsub_rn(p, pn)));                        // shift.add_(old - p)
+        float shift = R<true>(__fadd_rn(__bfloat162float(*sh), upd));               // shift.add_(update)
+        const float pn = R<true>(__fadd_rn(p, shift));                              // p.add_(shift)
+        shift = R<true>(__fadd_rn(shift, __fsub_rn(p, pn)));                        // shift.add_(old - p)
         *sh = __float2bfloat16_rn(shift);
         reinterpret_cast<__nv_bfloat16*>(T.p)[j] = __float2bfloat16_rn(pn);
       } else {
@@ -396,12 +340,12 @@ void fill(AmList& tl, const dpipe_automagic_tensor* t, int n, int* pos, long lon
     long long tiles = 0, fold = 0, lrow = 0;
     tl.rp[k] = tl.cp[k] = off;
     if (T.flags & DPIPE_AUTOMAGIC_FACTORED) {
-      const long long nstrip = (T.C + AM_TILE - 1) / AM_TILE, nrb = (T.R + AM_TILE - 1) / AM_TILE;
-      tiles = T.L * nrb * nstrip;
-      fold = (T.L * T.R + AM_THREADS - 1) / AM_THREADS + (T.L * T.C + AM_THREADS - 1) / AM_THREADS;
+      const FmGeom f{T.L, T.R, T.C};
+      tiles = f.tiles();
+      fold = f.fold_ctas(AM_THREADS);
       lrow = T.L;
-      tl.cp[k] = off + nstrip * T.L * T.R;
-      off = tl.cp[k] + nrb * T.L * T.C;
+      tl.cp[k] = off + f.row_partials();
+      off = tl.cp[k] + f.col_partials();
     }
     tl.tiles0[k + 1] = tl.tiles0[k] + tiles;
     tl.fold0[k + 1] = tl.fold0[k] + fold;

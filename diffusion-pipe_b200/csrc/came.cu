@@ -24,13 +24,13 @@
 #include <cuda_bf16.h>
 
 #include "host_util.h"
+#include "optim_common.cuh"
 
 namespace dpipe {
 namespace {
 
 constexpr int CM_MAX = 64;
 constexpr int CM_THREADS = 256;
-constexpr int CM_TILE = 128;            // tile: 128 rows (16 per warp) x 128 columns (4 per lane)
 constexpr long long CM_ELEMS = 8192;    // elements of one tensor per CTA of the per-element kernels
 
 struct CmList {
@@ -74,143 +74,43 @@ __device__ __forceinline__ double* sums_of(const dpipe_came_tensor& T, bool res)
   return T.sums + 1 + (res ? T.L * (T.R + T.C + 1) : 0);
 }
 
-template <bool BF16>
-__device__ __forceinline__ float R(float x) { return BF16 ? __bfloat162float(__float2bfloat16_rn(x)) : x; }
-__device__ __forceinline__ float rsqrt_rn(float x) { return __fdiv_rn(1.0f, __fsqrt_rn(x)); }   // 1 / sqrt(x)
-
-template <bool BF16>
-__device__ __forceinline__ float ld1(const void* __restrict__ a, long long j) {
-  return BF16 ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(a)[j]) : reinterpret_cast<const float*>(a)[j];
-}
-template <bool BF16>
-__device__ __forceinline__ void st1(void* __restrict__ a, long long j, float x) {   // x is a value of the dtype
-  if (BF16) reinterpret_cast<__nv_bfloat16*>(a)[j] = __float2bfloat16_rn(x);
-  else reinterpret_cast<float*>(a)[j] = x;
-}
-__device__ __forceinline__ float ldd(const void* a, long long j, int dt) { return dt == 0 ? ld1<true>(a, j) : ld1<false>(a, j); }
-__device__ __forceinline__ void std1(void* a, long long j, float x, int dt) {
-  if (dt == 0) st1<true>(a, j, x);
-  else st1<false>(a, j, x);
-}
-
-// element k of a 16-byte vector (8 bf16 or 4 fp32), and its replacement by a value of the dtype
-template <bool BF16>
-__device__ __forceinline__ float lane(const uint4& q, int k) {
-  const uint32_t w = (&q.x)[BF16 ? k >> 1 : k];
-  return BF16 ? __uint_as_float((k & 1) ? (w & 0xffff0000u) : (w << 16)) : __uint_as_float(w);
-}
-template <bool BF16>
-__device__ __forceinline__ void set_lane(uint4& q, int k, float x) {
-  uint32_t& w = (&q.x)[BF16 ? k >> 1 : k];
-  if (BF16) {
-    const uint32_t b = __float_as_uint(x) >> 16;
-    w = (k & 1) ? ((w & 0xffffu) | (b << 16)) : ((w & 0xffff0000u) | b);
-  } else {
-    w = __float_as_uint(x);
-  }
-}
-
-__device__ __forceinline__ int find(const long long* pre, int n, long long b) {
-  int lo = 0, hi = n - 1;                                   // last i with pre[i] <= b
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (pre[mid] <= b) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-  return v;
-}
-
-__device__ __forceinline__ double block_sum(double v, double* red) {   // fixed tree; valid in every thread
-  v = warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < CM_THREADS / 32; ++w) s += red[w];
-  return s;
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
 // factored statistics
 // ---------------------------------------------------------------------------------------------------------------------
-// one element of a tile: u0 = g*g + eps1 (second moment), or the momentum update and res = (u - m)^2 + eps2
+// one element of a tile: u0 = g*g + eps1 (second moment), or the momentum update and res = (u - m)^2 + eps2, from the
+// second moment's row and column factors
 template <bool BF16, bool RES>
-__device__ __forceinline__ float tile_elem(const dpipe_came_tensor& T, const Coef& k, long long j, float rf, float cf,
-                                           float clipdiv) {
-  const float g = ld1<BF16>(T.g, j);
-  if (!RES) return R<BF16>(__fadd_rn(R<BF16>(__fmul_rn(g, g)), k.eps1));
-  float u = R<BF16>(__fmul_rn(R<BF16>(__fmul_rn(rf, cf)), g));
-  u = R<BF16>(__fdiv_rn(u, clipdiv));
-  const float m = R<BF16>(__fmaf_rn(u, k.a1, R<BF16>(__fmul_rn(ld1<BF16>(T.m, j), k.b1))));
-  st1<BF16>(T.m, j, m);
-  const float d = R<BF16>(__fsub_rn(u, m));
-  return R<BF16>(__fadd_rn(R<BF16>(__fmul_rn(d, d)), k.eps2));
-}
-
-template <bool BF16, bool RES>
-__device__ __forceinline__ void tile(const CmList& tl, int i, long long b, double* __restrict__ scratch, double* colred) {
-  const dpipe_came_tensor& T = tl.t[i];
-  const Coef k = coef_of(T);
-  const long long R_ = T.R, C = T.C, LR = T.L * R_, LC = T.L * C;
-  const long long nstrip = (C + CM_TILE - 1) / CM_TILE, nrb = (R_ + CM_TILE - 1) / CM_TILE;
-  const long long strip = b % nstrip;
-  b /= nstrip;
-  const long long rb = b % nrb, l = b / nrb;
-  const int warp = threadIdx.x >> 5, ln = threadIdx.x & 31;
-  const float* rf = rfac(T, false) + l * R_;
-  const float* cf = cfac(T, false) + l * C;
-  const float clipdiv = RES ? T.fac[0] : 1.0f;
-  double cacc[4] = {0.0, 0.0, 0.0, 0.0};
-  const long long c0 = strip * CM_TILE + ln;
-  float cv[4];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) cv[j] = RES && c0 + 32 * j < C ? cf[c0 + 32 * j] : 0.f;
-#pragma unroll 1                                                             // unrolled, the u0 pass spills
-  for (int kk = 0; kk < CM_TILE / 8; ++kk) {
-    const long long r = rb * CM_TILE + warp + 8 * kk;
-    if (r >= R_) break;                                                      // warp-uniform
-    const long long base = (l * R_ + r) * C;
-    const float rv = RES ? rf[r] : 0.f;
-    double rs = 0.0;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      if (c0 + 32 * j < C) {
-        const double x = tile_elem<BF16, RES>(T, k, base + c0 + 32 * j, rv, cv[j], clipdiv);
-        rs += x;
-        cacc[j] += x;
-      }
-    }
-    rs = warp_sum(rs);
-    if (ln == 0) scratch[tl.rp[i] + strip * LR + l * R_ + r] = rs;
+struct TileElem {
+  const dpipe_came_tensor& T;
+  const Coef& k;
+  float clipdiv;
+  __device__ __forceinline__ float row(long long l, long long r) const { return RES ? rfac(T, false)[l * T.R + r] : 0.f; }
+  __device__ __forceinline__ float col(long long l, long long c) const { return RES ? cfac(T, false)[l * T.C + c] : 0.f; }
+  __device__ __forceinline__ float operator()(long long j, float rf, float cf) const {
+    const float g = ld1<BF16>(T.g, j);
+    if (!RES) return R<BF16>(__fadd_rn(R<BF16>(__fmul_rn(g, g)), k.eps1));
+    float u = R<BF16>(__fmul_rn(R<BF16>(__fmul_rn(rf, cf)), g));
+    u = R<BF16>(__fdiv_rn(u, clipdiv));
+    const float m = R<BF16>(__fmaf_rn(u, k.a1, R<BF16>(__fmul_rn(ld1<BF16>(T.m, j), k.b1))));
+    st1<BF16>(T.m, j, m);
+    const float d = R<BF16>(__fsub_rn(u, m));
+    return R<BF16>(__fadd_rn(R<BF16>(__fmul_rn(d, d)), k.eps2));
   }
-#pragma unroll
-  for (int j = 0; j < 4; ++j) colred[(threadIdx.x >> 5) * CM_TILE + ln + 32 * j] = cacc[j];
-  __syncthreads();
-  if (threadIdx.x < CM_TILE) {
-    const long long c = strip * CM_TILE + threadIdx.x;
-    if (c < C) {
-      double a = 0.0;
-      for (int w = 0; w < CM_THREADS / 32; ++w) a += colred[w * CM_TILE + threadIdx.x];
-      scratch[tl.cp[i] + rb * LC + l * C + c] = a;
-    }
-  }
-}
+};
 
 template <bool RES>
 __global__ void __launch_bounds__(CM_THREADS) cm_tile_kernel(const __grid_constant__ CmList tl,
                                                             double* __restrict__ scratch) {
-  __shared__ double colred[CM_THREADS / 32 * CM_TILE];
+  __shared__ double colred[CM_THREADS / 32 * FM_TILE];
   long long b = blockIdx.x;
   const int i = find(tl.tile0, tl.n, b);
+  const dpipe_came_tensor& T = tl.t[i];
   b -= tl.tile0[i];
-  if (tl.t[i].dtype == 0) tile<true, RES>(tl, i, b, scratch, colred);
-  else tile<false, RES>(tl, i, b, scratch, colred);
+  const FmGeom f{T.L, T.R, T.C};
+  const Coef k = coef_of(T);
+  const float clipdiv = RES ? T.fac[0] : 1.0f;
+  if (T.dtype == 0) fm_tile<CM_THREADS>(f, b, scratch, tl.rp[i], tl.cp[i], colred, TileElem<true, RES>{T, k, clipdiv});
+  else fm_tile<CM_THREADS>(f, b, scratch, tl.rp[i], tl.cp[i], colred, TileElem<false, RES>{T, k, clipdiv});
 }
 
 // one thread per row (then per column): fold the partials in a fixed order, EMA with beta (beta2 / beta3), column
@@ -225,12 +125,13 @@ __global__ void __launch_bounds__(CM_THREADS) cm_fold_kernel(const __grid_consta
   const float beta = res ? k.b3 : k.b2, alpha = res ? k.a3 : k.a2;
   const bool bf = T.dtype == 0;
   const long long R_ = T.R, C = T.C, LR = T.L * R_, LC = T.L * C;
+  const FmGeom f{T.L, R_, C};
   double* sums = sums_of(T, res);
-  const long long nrowcta = (LR + CM_THREADS - 1) / CM_THREADS;
+  const long long nrowcta = f.row_ctas(CM_THREADS);
   if (b < nrowcta) {
     const long long q = b * CM_THREADS + threadIdx.x;
     if (q >= LR) return;
-    const long long nstrip = (C + CM_TILE - 1) / CM_TILE;
+    const long long nstrip = f.nstrip();
     double a = 0.0;
     for (long long st = 0; st < nstrip; ++st) a += scratch[tl.rp[i] + st * LR + q];
     sums[q] = a;
@@ -238,22 +139,22 @@ __global__ void __launch_bounds__(CM_THREADS) cm_fold_kernel(const __grid_consta
     const float mean = __double2float_rn(a / (double)C);                     // x.mean(dim=-1)
     // row.mul_(beta).add_(mean, alpha=1-beta): torch's add with alpha is one fma; every op rounds to the dtype
     float r;
-    if (bf) r = R<true>(__fmaf_rn(R<true>(mean), alpha, R<true>(__fmul_rn(ldd(row, q, 0), beta))));
-    else r = __fmaf_rn(mean, alpha, __fmul_rn(ldd(row, q, 1), beta));
-    std1(row, q, r, T.dtype);
+    if (bf) r = R<true>(__fmaf_rn(R<true>(mean), alpha, R<true>(__fmul_rn(ld_dt(row, q, 0), beta))));
+    else r = __fmaf_rn(mean, alpha, __fmul_rn(ld_dt(row, q, 1), beta));
+    st_dt(row, q, r, T.dtype);
   } else {
     const long long q = (b - nrowcta) * CM_THREADS + threadIdx.x;
     if (q >= LC) return;
-    const long long nrb = (R_ + CM_TILE - 1) / CM_TILE;
+    const long long nrb = f.nrb();
     double a = 0.0;
     for (long long kk = 0; kk < nrb; ++kk) a += scratch[tl.cp[i] + kk * LC + q];
     sums[LR + q] = a;
     void* col = res ? T.res_col : T.col;
     const float mean = __double2float_rn(a / (double)R_);                    // x.mean(dim=-2)
     float c;
-    if (bf) c = R<true>(__fmaf_rn(R<true>(mean), alpha, R<true>(__fmul_rn(ldd(col, q, 0), beta))));
-    else c = __fmaf_rn(mean, alpha, __fmul_rn(ldd(col, q, 1), beta));
-    std1(col, q, c, T.dtype);
+    if (bf) c = R<true>(__fmaf_rn(R<true>(mean), alpha, R<true>(__fmul_rn(ld_dt(col, q, 0), beta))));
+    else c = __fmaf_rn(mean, alpha, __fmul_rn(ld_dt(col, q, 1), beta));
+    st_dt(col, q, c, T.dtype);
     cfac(T, res)[q] = bf ? R<true>(rsqrt_rn(c)) : rsqrt_rn(c);                // col.rsqrt()
   }
 }
@@ -269,14 +170,14 @@ __global__ void __launch_bounds__(CM_THREADS) cm_rowmean_kernel(const __grid_con
   const long long R_ = T.R;
   const void* row = res ? T.res_row : T.row;
   double a = 0.0;
-  for (long long kk = threadIdx.x; kk < R_; kk += CM_THREADS) a += ldd(row, l * R_ + kk, T.dtype);
-  a = block_sum(a, red);
+  for (long long kk = threadIdx.x; kk < R_; kk += CM_THREADS) a += ld_dt(row, l * R_ + kk, T.dtype);
+  a = block_sum<CM_THREADS>(a, red);
   if (threadIdx.x == 0) sums_of(T, res)[T.L * (R_ + T.C) + l] = a;
   float rm = __double2float_rn(a / (double)R_);
   if (bf) rm = R<true>(rm);
   float* rf = rfac(T, res) + l * R_;
   for (long long kk = threadIdx.x; kk < R_; kk += CM_THREADS) {
-    const float x = ldd(row, l * R_ + kk, T.dtype);
+    const float x = ld_dt(row, l * R_ + kk, T.dtype);
     rf[kk] = bf ? R<true>(rsqrt_rn(R<true>(__fdiv_rn(x, rm)))) : rsqrt_rn(__fdiv_rn(x, rm));
   }
 }
@@ -284,22 +185,12 @@ __global__ void __launch_bounds__(CM_THREADS) cm_rowmean_kernel(const __grid_con
 // ---------------------------------------------------------------------------------------------------------------------
 // per-element kernels: one CTA per CM_ELEMS elements of one tensor
 // ---------------------------------------------------------------------------------------------------------------------
+// p, g, m (and v of an unfactored tensor) go through 16-byte vectors when they share their offset mod 16 B
 __host__ __device__ __forceinline__ bool vectorised(const dpipe_came_tensor& T) {
   const uintptr_t mis = reinterpret_cast<uintptr_t>(T.p) & 15;
   return (reinterpret_cast<uintptr_t>(T.g) & 15) == mis && (reinterpret_cast<uintptr_t>(T.m) & 15) == mis &&
          (T.factored || (reinterpret_cast<uintptr_t>(T.v) & 15) == mis);
 }
-__host__ __device__ __forceinline__ long long head_of(const dpipe_came_tensor& T) {
-  if (!vectorised(T)) return 0;
-  const long long esz = T.dtype == 0 ? 2 : 4;
-  const long long h = (long long)((16 - (reinterpret_cast<uintptr_t>(T.p) & 15)) & 15) / esz;
-  return h < T.numel ? h : T.numel;
-}
-__host__ __device__ __forceinline__ long long ctas_of(const dpipe_came_tensor& T) {
-  const long long body = T.numel - head_of(T);
-  return body > CM_ELEMS ? (body + CM_ELEMS - 1) / CM_ELEMS : 1;
-}
-
 // the factor pair of flat element j of a factored tensor [L, R, C]: rf[q] with q = j / C and cf[l * C + j % C]
 struct Pos {
   long long q, c;
@@ -336,7 +227,7 @@ __device__ __forceinline__ float sumsq_at(const dpipe_came_tensor& T, const Coef
 template <bool BF16>
 __device__ __forceinline__ double sumsq_range(const dpipe_came_tensor& T, const Coef& k, long long b) {
   constexpr int VEC = BF16 ? 8 : 4;
-  const long long h = head_of(T), lo = h + b * CM_ELEMS;
+  const long long h = head_of(T, vectorised(T)), lo = h + b * CM_ELEMS;
   const long long hi = lo + CM_ELEMS < T.numel ? lo + CM_ELEMS : T.numel;
   double s = 0.0;
   if (!vectorised(T)) {
@@ -392,7 +283,7 @@ __global__ void __launch_bounds__(CM_THREADS) cm_sumsq_kernel(const __grid_const
   b -= tl.cta0[i];
   const Coef k = coef_of(T);
   double s = T.dtype == 0 ? sumsq_range<true>(T, k, b) : sumsq_range<false>(T, k, b);
-  s = block_sum(s, red);
+  s = block_sum<CM_THREADS>(s, red);
   if (threadIdx.x == 0) scratch[tl.pp + blockIdx.x] = s;
 }
 
@@ -405,7 +296,7 @@ __global__ void __launch_bounds__(CM_THREADS) cm_clip_kernel(const __grid_consta
   const dpipe_came_tensor& T = tl.t[i];
   double s = 0.0;
   for (long long kk = tl.cta0[i] + threadIdx.x; kk < tl.cta0[i + 1]; kk += CM_THREADS) s += scratch[tl.pp + kk];
-  s = block_sum(s, red);
+  s = block_sum<CM_THREADS>(s, red);
   if (threadIdx.x != 0) return;
   T.sums[0] = s;
   const bool bf = T.dtype == 0;
@@ -448,7 +339,7 @@ template <bool BF16>
 __device__ __forceinline__ void apply_range(const dpipe_came_tensor& T, const Coef& k, long long b) {
   constexpr int VEC = BF16 ? 8 : 4;
   const float clipdiv = T.fac[0];
-  const long long h = head_of(T), lo = h + b * CM_ELEMS;
+  const long long h = head_of(T, vectorised(T)), lo = h + b * CM_ELEMS;
   const long long hi = lo + CM_ELEMS < T.numel ? lo + CM_ELEMS : T.numel;
   if (!vectorised(T)) {
     for (long long j = lo + threadIdx.x; j < hi; j += CM_THREADS) apply_at<BF16>(T, k, clipdiv, j);
@@ -546,17 +437,17 @@ long long fill(CmList& tl, const dpipe_came_tensor* t, int n, int* pos) {
     long long tiles = 0, fold = 0, lrow = 0;
     tl.rp[k] = tl.cp[k] = off;
     if (T.factored) {
-      const long long nstrip = (T.C + CM_TILE - 1) / CM_TILE, nrb = (T.R + CM_TILE - 1) / CM_TILE;
-      tiles = T.L * nrb * nstrip;
-      fold = (T.L * T.R + CM_THREADS - 1) / CM_THREADS + (T.L * T.C + CM_THREADS - 1) / CM_THREADS;
+      const FmGeom f{T.L, T.R, T.C};
+      tiles = f.tiles();
+      fold = f.fold_ctas(CM_THREADS);
       lrow = T.L;
-      tl.cp[k] = off + nstrip * T.L * T.R;
-      off = tl.cp[k] + nrb * T.L * T.C;
+      tl.cp[k] = off + f.row_partials();
+      off = tl.cp[k] + f.col_partials();
     }
     tl.tile0[k + 1] = tl.tile0[k] + tiles;
     tl.fold0[k + 1] = tl.fold0[k] + fold;
     tl.lrow0[k + 1] = tl.lrow0[k] + lrow;
-    tl.cta0[k + 1] = tl.cta0[k] + ctas_of(T);
+    tl.cta0[k + 1] = tl.cta0[k] + ctas_of<CM_ELEMS>(T, vectorised(T));
   }
   tl.pp = off;
   return off + tl.cta0[tl.n];

@@ -17,6 +17,7 @@
 #include <cuda_bf16.h>
 
 #include "host_util.h"
+#include "optim_common.cuh"
 
 namespace dpipe {
 namespace {
@@ -67,75 +68,13 @@ __device__ __forceinline__ PgStep step_of(const double* __restrict__ blk, const 
   return o;
 }
 
-// the layout of one tensor set: elements before 16-byte alignment (vectorised sets only) and the CTAs it takes
+// a tensor set goes through 16-byte vectors when all six tensors share their offset mod 16 B
 __host__ __device__ __forceinline__ bool vectorised(const dpipe_prodigy_tensor& T) {
   const uintptr_t mis = reinterpret_cast<uintptr_t>(T.p) & 15;
   return (reinterpret_cast<uintptr_t>(T.g) & 15) == mis && (reinterpret_cast<uintptr_t>(T.p0) & 15) == mis &&
          (reinterpret_cast<uintptr_t>(T.s) & 15) == mis && (reinterpret_cast<uintptr_t>(T.m) & 15) == mis &&
          (reinterpret_cast<uintptr_t>(T.v) & 15) == mis;
 }
-__host__ __device__ __forceinline__ long long head_of(const dpipe_prodigy_tensor& T) {
-  if (!vectorised(T)) return 0;
-  const long long esz = T.dtype == 0 ? 2 : 4;
-  const long long h = (long long)((16 - (reinterpret_cast<uintptr_t>(T.p) & 15)) & 15) / esz;
-  return h < T.numel ? h : T.numel;
-}
-__host__ __device__ __forceinline__ long long ctas_of(const dpipe_prodigy_tensor& T) {
-  const long long body = T.numel - head_of(T);
-  return body > PG_ELEMS ? (body + PG_ELEMS - 1) / PG_ELEMS : 1;
-}
-
-__device__ __forceinline__ int find(const long long* pre, int n, long long b) {
-  int lo = 0, hi = n - 1;                                   // last i with pre[i] <= b
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (pre[mid] <= b) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
-__device__ __forceinline__ double block_sum(double v, double* red) {   // fixed tree; valid in every thread
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < PG_THREADS / 32; ++w) s += red[w];
-  return s;
-}
-
-template <bool BF16>
-__device__ __forceinline__ float R(float x) { return BF16 ? __bfloat162float(__float2bfloat16_rn(x)) : x; }
-
-template <bool BF16>
-__device__ __forceinline__ float ld1(const void* __restrict__ a, long long j) {
-  return BF16 ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(a)[j]) : reinterpret_cast<const float*>(a)[j];
-}
-template <bool BF16>
-__device__ __forceinline__ void st1(void* __restrict__ a, long long j, float x) {   // x is a value of the dtype
-  if (BF16) reinterpret_cast<__nv_bfloat16*>(a)[j] = __float2bfloat16_rn(x);
-  else reinterpret_cast<float*>(a)[j] = x;
-}
-
-// element k of a 16-byte vector (8 bf16 or 4 fp32), and its replacement by a value of the dtype
-template <bool BF16>
-__device__ __forceinline__ float lane(const uint4& q, int k) {
-  const uint32_t w = (&q.x)[BF16 ? k >> 1 : k];
-  return BF16 ? __uint_as_float((k & 1) ? (w & 0xffff0000u) : (w << 16)) : __uint_as_float(w);
-}
-template <bool BF16>
-__device__ __forceinline__ void set_lane(uint4& q, int k, float x) {
-  uint32_t& w = (&q.x)[BF16 ? k >> 1 : k];
-  if (BF16) {
-    const uint32_t b = __float_as_uint(x) >> 16;
-    w = (k & 1) ? ((w & 0xffffu) | (b << 16)) : ((w & 0xffff0000u) | b);
-  } else {
-    w = __float_as_uint(x);
-  }
-}
-
 struct StatCoef {
   float b1, b2, b3, am, av, as;
 };
@@ -166,7 +105,7 @@ template <bool BF16>
 __device__ __forceinline__ void stats_range(const dpipe_prodigy_tensor& T, long long b, const StatCoef& c, double& dot,
                                             double& asum) {
   constexpr int VEC = BF16 ? 8 : 4;
-  const long long h = head_of(T), lo = h + b * PG_ELEMS;
+  const long long h = head_of(T, vectorised(T)), lo = h + b * PG_ELEMS;
   const long long hi = lo + PG_ELEMS < T.numel ? lo + PG_ELEMS : T.numel;
   if (!vectorised(T)) {
     for (long long j = lo + threadIdx.x; j < hi; j += PG_THREADS) stat_at<BF16>(T, j, c, dot, asum);
@@ -218,8 +157,8 @@ __global__ void __launch_bounds__(PG_THREADS) pg_stats_kernel(const __grid_const
   double dot = 0.0, asum = 0.0;
   if (T.dtype == 0) stats_range<true>(T, b, c, dot, asum);
   else stats_range<false>(T, b, c, dot, asum);
-  dot = block_sum(dot, red);
-  asum = block_sum(asum, red);
+  dot = block_sum<PG_THREADS>(dot, red);
+  asum = block_sum<PG_THREADS>(asum, red);
   if (threadIdx.x == 0) {
     partials[2 * blockIdx.x] = dot;
     partials[2 * blockIdx.x + 1] = asum;
@@ -237,8 +176,8 @@ __global__ void __launch_bounds__(PG_THREADS) pg_fold_kernel(const __grid_consta
     dot += partials[2 * k];
     asum += partials[2 * k + 1];
   }
-  dot = block_sum(dot, red);
-  asum = block_sum(asum, red);
+  dot = block_sum<PG_THREADS>(dot, red);
+  asum = block_sum<PG_THREADS>(asum, red);
   if (threadIdx.x == 0) {
     sums[2 * tl.slot[i]] = dot;
     sums[2 * tl.slot[i] + 1] = asum;
@@ -287,7 +226,7 @@ __device__ __forceinline__ float apply_elem(float p, float m, float v, const App
 template <bool BF16>
 __device__ __forceinline__ void apply_range(const dpipe_prodigy_tensor& T, long long b, const ApplyCoef& c) {
   constexpr int VEC = BF16 ? 8 : 4;
-  const long long h = head_of(T), lo = h + b * PG_ELEMS;
+  const long long h = head_of(T, vectorised(T)), lo = h + b * PG_ELEMS;
   const long long hi = lo + PG_ELEMS < T.numel ? lo + PG_ELEMS : T.numel;
   if (!vectorised(T)) {
     for (long long j = lo + threadIdx.x; j < hi; j += PG_THREADS)
@@ -373,7 +312,7 @@ long long fill(PgList& tl, const dpipe_prodigy_tensor* t, int n, int* pos) {
     if (t[*pos].numel == 0) continue;
     tl.t[tl.n] = t[*pos];
     tl.slot[tl.n] = *pos;
-    tl.cta0[tl.n + 1] = tl.cta0[tl.n] + ctas_of(t[*pos]);
+    tl.cta0[tl.n + 1] = tl.cta0[tl.n] + ctas_of<PG_ELEMS>(t[*pos], vectorised(t[*pos]));
     ++tl.n;
   }
   return tl.cta0[tl.n];

@@ -22,6 +22,7 @@
 #include <cuda_bf16.h>
 
 #include "host_util.h"
+#include "optim_common.cuh"
 
 namespace dpipe {
 
@@ -181,52 +182,36 @@ struct AdamwScalars {
   float lr, beta1_comp, beta2_hat, one_minus_beta2_hat, eps, decay;
 };
 
-template <bool BF16>
-__device__ __forceinline__ float to_state(float x) {
-  return BF16 ? __bfloat162float(__float2bfloat16_rn(x)) : x;
-}
-
 // one element; p, m, v, c are exact values of the state dtype on entry and on exit
 template <bool BF16, bool KAHAN>
 __device__ __forceinline__ void adamw_elem(float& p, const float g, float& m, float& v, float& c, const AdamwScalars& s) {
-  p = to_state<BF16>(__fmul_rn(p, s.decay));                                     // p.mul_(1 - lr*wd)
+  p = R<BF16>(__fmul_rn(p, s.decay));                                            // p.mul_(1 - lr*wd)
   const float w = s.beta1_comp;                                                  // m.lerp_(g, w), torch's two-sided form
   const float d = __fsub_rn(g, m);
-  m = to_state<BF16>(fabsf(w) < 0.5f ? __fadd_rn(m, __fmul_rn(w, d)) : __fsub_rn(g, __fmul_rn(d, __fsub_rn(1.0f, w))));
-  v = to_state<BF16>(__fmul_rn(v, s.beta2_hat));                                 // v.mul_(beta2_hat)
-  v = to_state<BF16>(__fadd_rn(v, __fmul_rn(__fmul_rn(s.one_minus_beta2_hat, g), g)));   // .addcmul_(g, g, 1-beta2_hat)
-  const float den = to_state<BF16>(__fadd_rn(to_state<BF16>(__fsqrt_rn(v)), s.eps));      // v.sqrt().add_(eps)
+  m = R<BF16>(fabsf(w) < 0.5f ? __fadd_rn(m, __fmul_rn(w, d)) : __fsub_rn(g, __fmul_rn(d, __fsub_rn(1.0f, w))));
+  v = R<BF16>(__fmul_rn(v, s.beta2_hat));                                        // v.mul_(beta2_hat)
+  v = R<BF16>(__fadd_rn(v, __fmul_rn(__fmul_rn(s.one_minus_beta2_hat, g), g)));          // .addcmul_(g, g, 1-beta2_hat)
+  const float den = R<BF16>(__fadd_rn(R<BF16>(__fsqrt_rn(v)), s.eps));                    // v.sqrt().add_(eps)
   const float upd = __fdiv_rn(__fmul_rn(-s.lr, m), den);                         // addcdiv's value * m / den
   if (KAHAN) {
-    c = to_state<BF16>(__fadd_rn(c, upd));
+    c = R<BF16>(__fadd_rn(c, upd));
     const float old = p;
-    p = to_state<BF16>(__fadd_rn(p, c));
-    c = to_state<BF16>(__fadd_rn(c, to_state<BF16>(__fsub_rn(old, p))));
+    p = R<BF16>(__fadd_rn(p, c));
+    c = R<BF16>(__fadd_rn(c, R<BF16>(__fsub_rn(old, p))));
   } else {
-    p = to_state<BF16>(__fadd_rn(p, upd));
+    p = R<BF16>(__fadd_rn(p, upd));
   }
-}
-
-template <bool BF16>
-__device__ __forceinline__ float ld_elem(const void* a, long long j) {
-  return BF16 ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(a)[j]) : reinterpret_cast<const float*>(a)[j];
-}
-
-template <bool BF16>
-__device__ __forceinline__ void st_elem(void* a, long long j, float x) {
-  if (BF16) reinterpret_cast<__nv_bfloat16*>(a)[j] = __float2bfloat16_rn(x);
-  else reinterpret_cast<float*>(a)[j] = x;
 }
 
 template <bool BF16, bool KAHAN>
 __device__ __forceinline__ void adamw_scalar(const AdamwList& tl, int i, long long j, const AdamwScalars& s) {
-  float p = ld_elem<BF16>(tl.p[i], j), m = ld_elem<BF16>(tl.m[i], j), v = ld_elem<BF16>(tl.v[i], j);
-  float c = KAHAN ? ld_elem<BF16>(tl.c[i], j) : 0.f;
-  adamw_elem<BF16, KAHAN>(p, ld_elem<BF16>(tl.g[i], j), m, v, c, s);
-  st_elem<BF16>(tl.p[i], j, p);
-  st_elem<BF16>(tl.m[i], j, m);
-  st_elem<BF16>(tl.v[i], j, v);
-  if (KAHAN) st_elem<BF16>(tl.c[i], j, c);
+  float p = ld1<BF16>(tl.p[i], j), m = ld1<BF16>(tl.m[i], j), v = ld1<BF16>(tl.v[i], j);
+  float c = KAHAN ? ld1<BF16>(tl.c[i], j) : 0.f;
+  adamw_elem<BF16, KAHAN>(p, ld1<BF16>(tl.g[i], j), m, v, c, s);
+  st1<BF16>(tl.p[i], j, p);
+  st1<BF16>(tl.m[i], j, m);
+  st1<BF16>(tl.v[i], j, v);
+  if (KAHAN) st1<BF16>(tl.c[i], j, c);
 }
 
 // one 32-bit word of each of the five 16-byte vectors: two bf16 elements or one fp32 element, updated in place (the
